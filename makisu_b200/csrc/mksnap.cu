@@ -97,6 +97,8 @@ struct mksnap {
 
     TileRec *d_tiles = nullptr;
     CUtensorMap tm_main[MAX_SLOTS]; // per slot: arena viewed as [rows][128 B]
+    CUtensorMap tm_crc[MAX_SLOTS];  // the same with the box of the CRC variant's tiles
+    uint32_t *d_part = nullptr;     // CRC of every 128-byte arena row, written by the CRC variant of the scan
     int scan_cfg = 0; // index into SCAN_SHAPES
     bool sha_fma = true; // chunk SHA-256: additions on the FMA pipe
     uint32_t *d_pool = nullptr;
@@ -219,11 +221,20 @@ void build_crc_consts(CrcConsts *c)
     for (int l = 0; l < 32; l++)
         for (int k = 0; k < 4; k++)
             c->lane_c[l * 4 + k] = xpow_bits(32 + 8 * (508 - 16 * l - 4 * k));
-    uint32_t sq = 0x40000000u;
-    for (int i = 0; i < 32; i++) {
-        c->xp[i] = sq;
-        sq = crc_mulmod(sq, sq);
-    }
+    for (int t = 0; t < 4; t++)
+        for (uint32_t v = 0; v < 256; v++)
+            c->xe[t][v] = xpow_bits((uint64_t)v << (8 * t));
+    const uint32_t xg = xpow_bits(8ull * CRC_GRANULE * 128), x32 = xpow_bits(32);
+    for (int t = 0; t < 4; t++)
+        for (uint32_t v = 0; v < 256; v++) {
+            c->mulk_g[t][v] = crc_mulmod(v << (8 * t), xg);
+            c->mulk_w[t][v] = crc_mulmod(v << (8 * t), x32);
+        }
+    for (int l = 0; l < 32; l++)
+        for (int k = 0; k < 4; k++)
+            c->lane_g[l * 4 + k] = xpow_bits(32 + 8ull * CRC_GRANULE * (127 - 4 * l - k));
+    for (int j = 0; j < 32; j++)
+        c->word_g[j] = xpow_bits(32ull * (31 - j));
 }
 
 // generic device exclusive scan (u32), in -> out (may alias), n elements
@@ -419,13 +430,15 @@ static int alloc_table_buffers(mksnap *h, uint64_t rows)
     return 0;
 }
 
-template <int GROUPS, int TW, int ST> static int launch_scan(mksnap *h, uint32_t slot, uint32_t n_regions, cudaStream_t sk)
+template <int GROUPS, int TW, int ST, int REP = 0>
+static int launch_scan(mksnap *h, uint32_t slot, uint32_t n_regions, cudaStream_t sk)
 {
-    using Cfg = ScanCfg<GROUPS, TW, ST>;
+    using Cfg = ScanCfg<GROUPS, TW, ST, REP>;
     const uint32_t n_tiles = (n_regions + Cfg::TILE_WARPS - 1) / Cfg::TILE_WARPS;
     const uint32_t grid = std::min<uint32_t>(n_tiles, (uint32_t)h->sm_count);
-    k_roll_scan<GROUPS, TW, ST><<<grid, Cfg::THREADS, Cfg::SMEM, sk>>>(h->tm_main[slot], n_tiles, h->prm.strict_lim, h->prm.loose_lim,
-                                                                     h->d_tiles, h->d_pool, h->pool_cap, h->d_pool_count, &h->d_sc->err);
+    k_roll_scan<GROUPS, TW, ST, REP><<<grid, Cfg::THREADS, Cfg::SMEM, sk>>>(
+        REP ? h->tm_crc[slot] : h->tm_main[slot], n_tiles, h->prm.strict_lim, h->prm.loose_lim, h->d_tiles, h->d_pool,
+        h->pool_cap, h->d_pool_count, &h->d_sc->err, &h->d_consts->mulk_w[0][0], h->d_part);
     LAUNCH_OK(h);
     return 0;
 }
@@ -450,6 +463,11 @@ static int launch_scan_cfg(mksnap *h, uint32_t slot, uint32_t n_regions, cudaStr
     default: return launch_scan<4, 6, 8>(h, slot, n_regions, sk);
     }
 }
+
+// The CRC variant of the scan (submits with CRC extents and CDC files): 3 groups x 6 warps per tile, 6 stages, tables in 16 copies
+// (64 KiB: lanes l and l+16 share one, at most a 2-way conflict).  Fastest of the shapes measured on an H100 (DESIGN.md
+// section 5); full replication (128 KiB) leaves too little room for stages.
+#define MK_CRC_SCAN_SHAPE 3, 6, 6, 16
 
 extern "C" {
 
@@ -518,6 +536,7 @@ static int create_impl(mksnap *h)
 
     const uint64_t n_tiles = c.device_arena_bytes / SCAN_TILE + 128; // one TileRec per 4 KiB region (+ tile round-up)
     CK(h, cudaMalloc(&h->d_tiles, n_tiles * sizeof(TileRec)));
+    CK(h, cudaMalloc(&h->d_part, n_tiles * (SCAN_TILE / CRC_GRANULE) * 4)); // one u32 per row of every scanned region
     {
         EncodeTiledFn enc = nullptr;
         cudaDriverEntryPointQueryResult qres;
@@ -533,11 +552,15 @@ static int create_impl(mksnap *h)
             int rc;
             if ((rc = make_row_map(h, enc, &h->tm_main[s], h->d_slot[s], n_rows, box_rows)))
                 return rc;
+            if ((rc = make_row_map(h, enc, &h->tm_crc[s], h->d_slot[s], n_rows, ScanCfg<MK_CRC_SCAN_SHAPE>::BOX_ROWS)))
+                return rc;
         }
 #define MK_SET_SMEM(I, G, T, S) \
     CK(h, cudaFuncSetAttribute(k_roll_scan<G, T, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)ScanCfg<G, T, S>::SMEM));
         MK_SCAN_SHAPES(MK_SET_SMEM)
 #undef MK_SET_SMEM
+        CK(h, cudaFuncSetAttribute(k_roll_scan<MK_CRC_SCAN_SHAPE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                   (int)ScanCfg<MK_CRC_SCAN_SHAPE>::SMEM));
         const char *e2 = getenv("MKSNAP_SHA_FMA"); // tuning knob: 0 = plain adds in the chunk SHA-256 kernel
         if (e2 && e2[0] == '0')
             h->sha_fma = false;
@@ -663,7 +686,7 @@ void mksnap_destroy(mksnap_t *h)
     cudaFree(h->d_consts); cudaFree(h->d_sc); cudaFreeHost(h->h_sc);
     cudaFree(h->d_carry);
     cudaFree(h->d_crc_session);
-    cudaFree(h->d_tiles); cudaFree(h->d_pool); cudaFree(h->d_pool_count); cudaFree(h->d_counts); cudaFree(h->d_bases);
+    cudaFree(h->d_tiles); cudaFree(h->d_part); cudaFree(h->d_pool); cudaFree(h->d_pool_count); cudaFree(h->d_counts); cudaFree(h->d_bases);
     cudaFree(h->d_scan_tmp);
     cudaFree(h->d_order); cudaFree(h->d_chunk_start); cudaFree(h->d_chunk_len); cudaFree(h->d_chunk_end); cudaFree(h->d_digests);
     cudaFree(h->d_stream_digests); cudaFree(h->d_stream_state);
@@ -889,12 +912,24 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         k_carry_in<<<1, 256, 0, sk>>>(h->d_carry, d_arena, cont_off, m.d_files, 0u, h->d_sc);
         LAUNCH_OK(h);
     }
+    // the scan comes first: with CRC extents in the submit it also leaves the CRC of every arena row in d_part, and
+    // K0 combines those instead of reading the arena a second time
     CK(h, cudaEventRecord(h->ev[0], sk));
+    if (n_files) {
+        const uint32_t n_regions = (uint32_t)((used + SCAN_TILE - 1) / SCAN_TILE);
+        CK(h, cudaMemsetAsync(h->d_pool_count, 0, 4, sk));
+        int rc = n_crc && pieces ? launch_scan<MK_CRC_SCAN_SHAPE>(h, slot, n_regions, sk)
+                                 : launch_scan_cfg(h, slot, n_regions, sk);
+        if (rc)
+            return rc;
+    }
+    CK(h, cudaEventRecord(h->ev[1], sk));
     if (n_crc && pieces) {
         const uint32_t grid = (uint32_t)std::min<uint64_t>(h->sm_count, (pieces + 31) / 32);
         CK(h, cudaMemsetAsync(m.d_ext_pure, 0, n_crc * 4, sk));
         k_crc32_extents<<<grid, CRC_THREADS, CRC_SMEM, sk>>>(d_arena, m.d_crc, m.d_piece_base, (uint32_t)n_crc,
-                                                            (uint32_t)pieces, h->d_consts, m.d_ext_pure, &h->d_sc->crc_acc);
+                                                            (uint32_t)pieces, h->d_consts, m.d_ext_pure, &h->d_sc->crc_acc,
+                                                            n_files ? h->d_part : nullptr);
         LAUNCH_OK(h);
     }
     if (n_crc) { // pure(extent) of this submit's extents joins the session table (zero-length extents keep their slot)
@@ -904,14 +939,6 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
             CK(h, cudaMemcpyAsync(h->d_crc_session + h->crc_session_n, m.d_ext_pure,
                                   std::min<uint64_t>(n_crc, h->crc_session_cap - h->crc_session_n) * 4, cudaMemcpyDeviceToDevice, sk));
         h->crc_session_n += n_crc;
-    }
-    CK(h, cudaEventRecord(h->ev[1], sk));
-    if (n_files) {
-        const uint32_t n_regions = (uint32_t)((used + SCAN_TILE - 1) / SCAN_TILE);
-        CK(h, cudaMemsetAsync(h->d_pool_count, 0, 4, sk));
-        int rc = launch_scan_cfg(h, slot, n_regions, sk);
-        if (rc)
-            return rc;
     }
     CK(h, cudaEventRecord(h->ev[2], sk));
     if (n_files) {
@@ -1236,8 +1263,8 @@ int mksnap_stats(mksnap_t *h, mksnap_stats_t *out)
         float t[5];
         for (int i = 0; i < 5; i++)
             CK(h, cudaEventElapsedTime(&t[i], h->ev[i], h->ev[i + 1]));
-        h->stats.ms_crc = t[0];
-        h->stats.ms_scan = t[1];
+        h->stats.ms_scan = t[0];
+        h->stats.ms_crc = t[1];
         h->stats.ms_select = t[2];
         h->stats.ms_sha = t[3];
         h->stats.ms_stream = t[4];

@@ -1,7 +1,7 @@
 // mksnap_kernels.cuh — hand-written sm_90a kernels of the snapshot+hash path.
 //
-//   K0  k_crc32_extents   CRC-32/IEEE of the context stream      (HBM-read bound)
-//   K1  k_roll_scan       Roll-32 candidate scan                 (HBM-read bound)
+//   K0  k_crc32_extents   CRC-32/IEEE of the context stream      (HBM-read bound, or a combine of K1's row CRCs)
+//   K1  k_roll_scan       Roll-32 candidate scan [+ row CRCs]    (HBM-read bound)
 //   K1b k_select_cuts     min/normal/max cut selection per file  (latency, tiny)
 //   K2  k_sha256_ranges   SHA-256 of many byte ranges            (int-ALU bound)
 //       (the same kernel digests the serial layer-tar streams, K4, and the
@@ -132,6 +132,14 @@ __global__ void k_synth_fill(uint64_t *dst, uint64_t word0, uint64_t nwords, uin
 // coalesced uint4, chain step  acc = acc*x^4096 mod P  ^ word  done with four
 // byte-indexed table lookups.  The tables are replicated per lane in shared
 // memory ([4][256][32] words = 128 KiB) so every lookup is bank-conflict free.
+//
+// When the submit also ran the scan, the scan has left the CRC of every 128-byte
+// arena row in `part` (k_roll_scan<.., REP > 0>), and K0 reads those instead of the
+// bytes: a granule value h with pure(row) = h*x^32 behaves exactly like a word
+// whose last byte is the row's last byte, so the same chains, steps and fold work
+// on granules, with constants for a 128-byte element instead of a 4-byte one
+// (a warp row = 128 granules = 16 KiB of data).  A first or last granule only
+// partly inside its piece is computed from the arena bytes.
 // ------------------------------------------------------------------------
 struct CrcExtent {
     uint64_t off;    // byte offset in the slot, multiple of 16
@@ -143,10 +151,16 @@ constexpr uint32_t CRC_PIECE = 256u * 1024u; // bytes per warp-piece (multiple o
 constexpr int CRC_THREADS = 1024;
 constexpr size_t CRC_SMEM = 4u * 256u * 32u * sizeof(uint32_t);
 
+constexpr uint32_t CRC_GRANULE = 128; // bytes per partial CRC the scan writes (one arena row)
+
 struct CrcConsts {
-    uint32_t mulk[4][256]; // byte tables for a -> a*x^4096 mod P
-    uint32_t lane_c[128];  // x^(32 + 8*(508-16l-4c)) for (l,c)
-    uint32_t xp[32];       // x^(2^i), i = bit exponent
+    uint32_t mulk[4][256];   // byte tables for a -> a*x^4096 mod P
+    uint32_t lane_c[128];    // x^(32 + 8*(508-16l-4c)) for (l,c)
+    uint32_t xe[4][256];     // x^(v << 8t): x^E = product over the bytes t of E of xe[t][byte t]
+    uint32_t mulk_g[4][256]; // granule chains: a -> a*x^(8*128*128) mod P
+    uint32_t lane_g[128];    //   x^(32 + 8*128*(127-4l-c)) for (l,c)
+    uint32_t word_g[32];     // x^(32*(31-j)): word j of a granule -> its granule value
+    uint32_t mulk_w[4][256]; // the scan's per-row chains: a -> a*x^32 mod P
 };
 
 __device__ __forceinline__ uint32_t crc_step(uint32_t T, uint32_t a, uint32_t w)
@@ -163,11 +177,14 @@ __global__ void __launch_bounds__(CRC_THREADS, 1)
 k_crc32_extents(const uint8_t *__restrict__ arena, const CrcExtent *__restrict__ ext,
                 const uint32_t *__restrict__ piece_base, uint32_t n_ext, uint32_t n_pieces,
                 const CrcConsts *__restrict__ cst, uint32_t *__restrict__ ext_pure /* [n_ext], zeroed: pure(extent) */,
-                uint32_t *__restrict__ acc_out /* pure(stream) accumulator */)
+                uint32_t *__restrict__ acc_out /* pure(stream) accumulator */,
+                const uint32_t *__restrict__ part /* granule values of the scan, or null: read the bytes */)
 {
     extern __shared__ uint32_t s_tab[];
+    const uint32_t *const mulk = part ? &cst->mulk_g[0][0] : &cst->mulk[0][0];
+    const uint32_t *const lane_c = part ? cst->lane_g : cst->lane_c;
     for (uint32_t i = threadIdx.x; i < 4u * 256u * 32u; i += blockDim.x)
-        s_tab[i] = (&cst->mulk[0][0])[i >> 5];
+        s_tab[i] = mulk[i >> 5];
     __syncthreads();
 
     const uint32_t lane = threadIdx.x & 31;
@@ -190,44 +207,97 @@ k_crc32_extents(const uint8_t *__restrict__ arena, const CrcExtent *__restrict__
         const uint64_t start = (uint64_t)(piece - __ldg(piece_base + lo)) * CRC_PIECE;
         const uint64_t left = e.len - start;
         const uint32_t valid = left < CRC_PIECE ? (uint32_t)left : CRC_PIECE;
-        const uint32_t rows = (valid + 511u) >> 9;
-        const uint8_t *base = arena + e.off + start + lane * 16u;
-
+        uint32_t rows, pad; // chain rows of the piece; zero bytes after the piece to the end of the last row
         uint32_t a0 = 0, a1 = 0, a2 = 0, a3 = 0;
-        uint32_t r = 0;
-        // full rows, 4 loads in flight per lane
-        const uint32_t full_rows = valid >> 9;
-        for (; r + 4 <= full_rows; r += 4) {
-            uint4 w0 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)r * 512));
-            uint4 w1 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 1) * 512));
-            uint4 w2 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 2) * 512));
-            uint4 w3 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 3) * 512));
-            a0 = crc_step(T, a0, w0.x); a1 = crc_step(T, a1, w0.y); a2 = crc_step(T, a2, w0.z); a3 = crc_step(T, a3, w0.w);
-            a0 = crc_step(T, a0, w1.x); a1 = crc_step(T, a1, w1.y); a2 = crc_step(T, a2, w1.z); a3 = crc_step(T, a3, w1.w);
-            a0 = crc_step(T, a0, w2.x); a1 = crc_step(T, a1, w2.y); a2 = crc_step(T, a2, w2.z); a3 = crc_step(T, a3, w2.w);
-            a0 = crc_step(T, a0, w3.x); a1 = crc_step(T, a1, w3.y); a2 = crc_step(T, a2, w3.z); a3 = crc_step(T, a3, w3.w);
-        }
-        for (; r < rows; ++r) {
-            // remaining rows; the last one may be partial: bytes past `valid` count as zero
-            uint4 w = make_uint4(0, 0, 0, 0);
-            const int32_t nb = (int32_t)valid - (int32_t)(r * 512u + lane * 16u);
-            if (nb > 0) {
-                w = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)r * 512));
-                if (nb < 16) {
-                    uint32_t m[4];
+        if (part) {
+            // granules g = 0.. of the run that starts at S (512-aligned: lane l loads granules 4l..4l+3 of a row as one
+            // uint4).  Granules before gA and after gE lie outside the piece and count as zero.  When gA or gE is only
+            // partly inside it, lanes 0-7 compute gA and lanes 8-15 gE from the bytes, the zero-extended word j of a
+            // granule contributing word*x^(32*(31-j)).  Leading zero bytes do not change a pure CRC, trailing ones are
+            // `pad`.
+            const uint64_t A = e.off + start, Z = A + valid, S = A & ~511ull;
+            const uint32_t gA = (uint32_t)((A - S) / CRC_GRANULE), gE = (uint32_t)((Z - 1 - S) / CRC_GRANULE);
+            const bool cutA = A % CRC_GRANULE != 0, cutE = Z % CRC_GRANULE != 0;
+            uint32_t hg = 0;
+            if ((cutA || cutE) && lane < 16) {
+                const uint64_t q = S + (uint64_t)(lane < 8 ? gA : gE) * CRC_GRANULE + (lane & 7u) * 16u;
+                uint4 w = make_uint4(0, 0, 0, 0);
+                if (q >= A && q < Z) {
+                    w = ldg_stream(reinterpret_cast<const uint4 *>(arena + q));
+                    const uint64_t nb = Z - q;
+                    if (nb < 16) {
+                        uint32_t m[4];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) {
-                        int32_t bytes = nb - 4 * k;
-                        m[k] = bytes >= 4 ? 0xFFFFFFFFu : (bytes <= 0 ? 0u : (0xFFFFFFFFu >> (32 - 8 * bytes)));
+                        for (int k = 0; k < 4; ++k) {
+                            int32_t bytes = (int32_t)nb - 4 * k;
+                            m[k] = bytes >= 4 ? 0xFFFFFFFFu : (bytes <= 0 ? 0u : (0xFFFFFFFFu >> (32 - 8 * bytes)));
+                        }
+                        w.x &= m[0]; w.y &= m[1]; w.z &= m[2]; w.w &= m[3];
                     }
-                    w.x &= m[0]; w.y &= m[1]; w.z &= m[2]; w.w &= m[3];
                 }
+                const uint32_t *wg = cst->word_g + (lane & 7u) * 4u;
+                hg = crc_mulmod(w.x, wg[0]) ^ crc_mulmod(w.y, wg[1]) ^ crc_mulmod(w.z, wg[2]) ^ crc_mulmod(w.w, wg[3]);
             }
-            a0 = crc_step(T, a0, w.x); a1 = crc_step(T, a1, w.y); a2 = crc_step(T, a2, w.z); a3 = crc_step(T, a3, w.w);
+#pragma unroll
+            for (int s = 1; s < 8; s <<= 1)
+                hg ^= __shfl_xor_sync(0xFFFFFFFFu, hg, s);
+            const uint32_t hA = __shfl_sync(0xFFFFFFFFu, hg, 0), hE = __shfl_sync(0xFFFFFFFFu, hg, 8);
+            rows = (gE + 128u) / 128u;
+            pad = (uint32_t)(S + (uint64_t)rows * 128u * CRC_GRANULE - Z);
+            const uint32_t *pg = part + S / CRC_GRANULE;
+            for (uint32_t r = 0; r < rows; ++r) {
+                const uint32_t i0 = r * 128u + lane * 4u;
+                uint4 p = make_uint4(0, 0, 0, 0);
+                if (i0 <= gE)
+                    p = ldg_stream(reinterpret_cast<const uint4 *>(pg + i0));
+                uint32_t v[4] = {p.x, p.y, p.z, p.w};
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t i = i0 + k;
+                    v[k] = (i == gA && cutA) ? hA : (i == gE && cutE) ? hE : (i < gA || i > gE) ? 0u : v[k];
+                }
+                a0 = crc_step(T, a0, v[0]); a1 = crc_step(T, a1, v[1]); a2 = crc_step(T, a2, v[2]); a3 = crc_step(T, a3, v[3]);
+            }
+        } else {
+            rows = (valid + 511u) >> 9;
+            pad = rows * 512u - valid;
+            const uint8_t *base = arena + e.off + start + lane * 16u;
+            uint32_t r = 0;
+            // full rows, 4 loads in flight per lane
+            const uint32_t full_rows = valid >> 9;
+            for (; r + 4 <= full_rows; r += 4) {
+                uint4 w0 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)r * 512));
+                uint4 w1 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 1) * 512));
+                uint4 w2 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 2) * 512));
+                uint4 w3 = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)(r + 3) * 512));
+                a0 = crc_step(T, a0, w0.x); a1 = crc_step(T, a1, w0.y); a2 = crc_step(T, a2, w0.z); a3 = crc_step(T, a3, w0.w);
+                a0 = crc_step(T, a0, w1.x); a1 = crc_step(T, a1, w1.y); a2 = crc_step(T, a2, w1.z); a3 = crc_step(T, a3, w1.w);
+                a0 = crc_step(T, a0, w2.x); a1 = crc_step(T, a1, w2.y); a2 = crc_step(T, a2, w2.z); a3 = crc_step(T, a3, w2.w);
+                a0 = crc_step(T, a0, w3.x); a1 = crc_step(T, a1, w3.y); a2 = crc_step(T, a2, w3.z); a3 = crc_step(T, a3, w3.w);
+            }
+            for (; r < rows; ++r) {
+                // remaining rows; the last one may be partial: bytes past `valid` count as zero
+                uint4 w = make_uint4(0, 0, 0, 0);
+                const int32_t nb = (int32_t)valid - (int32_t)(r * 512u + lane * 16u);
+                if (nb > 0) {
+                    w = ldg_stream(reinterpret_cast<const uint4 *>(base + (size_t)r * 512));
+                    if (nb < 16) {
+                        uint32_t m[4];
+#pragma unroll
+                        for (int k = 0; k < 4; ++k) {
+                            int32_t bytes = nb - 4 * k;
+                            m[k] = bytes >= 4 ? 0xFFFFFFFFu : (bytes <= 0 ? 0u : (0xFFFFFFFFu >> (32 - 8 * bytes)));
+                        }
+                        w.x &= m[0]; w.y &= m[1]; w.z &= m[2]; w.w &= m[3];
+                    }
+                }
+                a0 = crc_step(T, a0, w.x); a1 = crc_step(T, a1, w.y); a2 = crc_step(T, a2, w.z); a3 = crc_step(T, a3, w.w);
+            }
         }
-        // fold the 128 chains of the warp: chain (l,c) ends 8*(508-16l-4c) bits before the row end
-        uint32_t c = crc_mulmod(a0, cst->lane_c[lane * 4 + 0]) ^ crc_mulmod(a1, cst->lane_c[lane * 4 + 1]) ^
-                     crc_mulmod(a2, cst->lane_c[lane * 4 + 2]) ^ crc_mulmod(a3, cst->lane_c[lane * 4 + 3]);
+        // fold the 128 chains of the warp: chain (l,c) ends 8*(508-16l-4c) bits (granules: 8*128*(127-4l-c)) before
+        // the row end
+        uint32_t c = crc_mulmod(a0, lane_c[lane * 4 + 0]) ^ crc_mulmod(a1, lane_c[lane * 4 + 1]) ^
+                     crc_mulmod(a2, lane_c[lane * 4 + 2]) ^ crc_mulmod(a3, lane_c[lane * 4 + 3]);
 #pragma unroll
         for (int s = 16; s; s >>= 1)
             c ^= __shfl_xor_sync(0xFFFFFFFFu, c, s);
@@ -237,25 +307,21 @@ k_crc32_extents(const uint8_t *__restrict__ arena, const CrcExtent *__restrict__
         // first to the END OF THE EXTENT: pure(extent) is kept per extent so that the host can remember it per file and
         // fold unchanged files into a later build's cacheID without sending their bytes (mksnap_crc_add) ...
         const uint32_t M = 0xFFFFFFFFu;
-        const uint32_t pad = rows * 512u - valid;
         const uint64_t after = left - valid;
         uint32_t E = (uint32_t)(((after % M) * 8ull) % M);
         E = (uint32_t)(((uint64_t)E + M - 8ull * pad) % M);
-        uint32_t f = ((E >> lane) & 1u) ? cst->xp[lane] : 0x80000000u;
-#pragma unroll
-        for (int s = 16; s; s >>= 1)
-            f = crc_mulmod(f, __shfl_xor_sync(0xFFFFFFFFu, f, s));
-        const uint32_t v = crc_mulmod(c, f);
+        // ... and on to its place in the stream: x^(8 * bytes after the extent) further.  Lanes 0-3 build x^E and lanes
+        // 4-7 x^(E + 8*suffix), each lane one byte-table factor, two rounds of products, then one multiplication by c
+        const uint32_t E2 = (uint32_t)(((uint64_t)E + ((e.suffix % M) * 8ull) % M) % M);
+        const uint32_t ex = lane < 4 ? E : E2;
+        uint32_t f = lane < 8 ? cst->xe[lane & 3][(ex >> (8 * (lane & 3))) & 255u] : 0x80000000u;
+        f = crc_mulmod(f, __shfl_xor_sync(0xFFFFFFFFu, f, 1));
+        f = crc_mulmod(f, __shfl_xor_sync(0xFFFFFFFFu, f, 2));
+        const uint32_t g = crc_mulmod(c, f);
+        const uint32_t v = __shfl_sync(0xFFFFFFFFu, g, 0);
         if (lane == 0 && v)
             atomicXor(ext_pure + lo, v);
-        // ... then on to its place in the stream: x^(8 * bytes after the extent); two exponentiations per 256 KiB piece
-        // cost little next to the piece itself; a separate pass over the extents would cost a launch and a read of them all
-        const uint32_t E2 = (uint32_t)(((e.suffix % M) * 8ull) % M);
-        uint32_t f2 = ((E2 >> lane) & 1u) ? cst->xp[lane] : 0x80000000u;
-#pragma unroll
-        for (int s = 16; s; s >>= 1)
-            f2 = crc_mulmod(f2, __shfl_xor_sync(0xFFFFFFFFu, f2, s));
-        warp_acc ^= crc_mulmod(v, f2);
+        warp_acc ^= __shfl_sync(0xFFFFFFFFu, g, 4);
     }
     if (lane == 0 && warp_acc)
         atomicXor(acc_out, warp_acc);
@@ -362,7 +428,9 @@ __device__ __forceinline__ uint32_t roll_step(uint32_t h, uint32_t u)
 // the HBM bandwidth x ~1 us of loaded latency.  With no table in shared memory all 227 KiB hold stages.
 // Shared-memory plan (dynamic region, 1 KiB aligned): STAGES stages of PITCH bytes (box rounded up to whole swizzle
 // atoms), then the mbarriers.
-template <int SCAN_GROUPS, int TW = 6, int ST = 8> struct ScanCfg {
+// The CRC variant (REP > 0) also keeps the slicing-by-4 tables of the per-row CRC chain after the stages, REP copies of
+// each entry: lane l reads copy l % REP.
+template <int SCAN_GROUPS, int TW = 6, int ST = 8, int REP = 0> struct ScanCfg {
     static constexpr uint32_t STAGES = ST;
     static constexpr uint32_t TILE_WARPS = TW;
     static constexpr uint32_t GROUPS = SCAN_GROUPS;
@@ -372,7 +440,9 @@ template <int SCAN_GROUPS, int TW = 6, int ST = 8> struct ScanCfg {
     static constexpr uint32_t PITCH = (TILE_BYTES + 1023) / 1024 * 1024;
     static constexpr uint32_t CONSUMER_WARPS = SCAN_GROUPS * TILE_WARPS;
     static constexpr uint32_t THREADS = (CONSUMER_WARPS + 1) * 32;
-    static constexpr uint32_t BARS_OFF = STAGES * PITCH;
+    static constexpr uint32_t TAB_OFF = STAGES * PITCH;
+    static constexpr uint32_t TAB_BYTES = 4u * 256u * REP * 4u;
+    static constexpr uint32_t BARS_OFF = TAB_OFF + TAB_BYTES;
     static constexpr uint32_t SMEM = BARS_OFF + 2 * STAGES * 8 + 1024; // dynamic bytes to request, alignment slack included
     static_assert(BOX_ROWS <= 256, "one TMA box");
     // Each stage must always be consumed by the same group.  Otherwise a group can reach a stage while its full barrier
@@ -381,13 +451,27 @@ template <int SCAN_GROUPS, int TW = 6, int ST = 8> struct ScanCfg {
     static_assert(SMEM <= 227 * 1024, "exceeds the 227 KiB per-CTA limit");
 };
 
-template <int SCAN_GROUPS, int TW, int ST>
+// a*x^32 ^ w with REP-fold replicated byte tables (table t, value v, copy k at word (t*256 + v)*REP + k)
+template <int REP> __device__ __forceinline__ uint32_t crc_step_rep(uint32_t T, uint32_t a, uint32_t w)
+{
+    const uint32_t r0 = lds_u32(byte_of<0>(a) * (4u * REP) + T);
+    const uint32_t r1 = lds_u32(byte_of<1>(a) * (4u * REP) + (T + 1024u * REP));
+    const uint32_t r2 = lds_u32(byte_of<2>(a) * (4u * REP) + (T + 2048u * REP));
+    const uint32_t r3 = lds_u32(byte_of<3>(a) * (4u * REP) + (T + 3072u * REP));
+    return r0 ^ r1 ^ r2 ^ r3 ^ w;
+}
+
+// REP > 0: the CRC variant.  Besides the candidates, every consumer thread runs a CRC chain h = h*x^32 ^ word over the
+// 32 words of its row as they pass through the roll, and writes h (pure(row) = h*x^32) to part[global row]: K0 then
+// takes whole rows of an extent from `part` instead of reading the arena a second time.
+template <int SCAN_GROUPS, int TW, int ST, int REP = 0>
 __global__ void __launch_bounds__((SCAN_GROUPS * TW + 1) * 32, 1)
 k_roll_scan(const __grid_constant__ CUtensorMap tm_main, uint32_t n_tiles, uint32_t strict_lim, uint32_t loose_lim,
             TileRec *__restrict__ tiles, uint32_t *__restrict__ pool, uint32_t pool_cap,
-            uint32_t *__restrict__ pool_count, uint32_t *__restrict__ err_flag)
+            uint32_t *__restrict__ pool_count, uint32_t *__restrict__ err_flag,
+            const uint32_t *__restrict__ crc_tab /* [4][256] a -> a*x^32 (REP > 0) */, uint32_t *__restrict__ part)
 {
-    using Cfg = ScanCfg<SCAN_GROUPS, TW, ST>;
+    using Cfg = ScanCfg<SCAN_GROUPS, TW, ST, REP>;
     constexpr uint32_t STAGES = Cfg::STAGES;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t s0 = (smem_u32(smem_raw) + 1023u) & ~1023u; // swizzle atoms are 1 KiB: align the stages ourselves
@@ -395,6 +479,11 @@ k_roll_scan(const __grid_constant__ CUtensorMap tm_main, uint32_t n_tiles, uint3
     const uint32_t bar_full = s0 + Cfg::BARS_OFF, bar_empty = bar_full + STAGES * 8;
     const uint32_t strict_thr = 0u - strict_lim, loose_thr = 0u - loose_lim; // top `bits` bits all ones
 
+    if constexpr (REP > 0) {
+        uint32_t *tab = reinterpret_cast<uint32_t *>(smem_raw + (s0 - smem_u32(smem_raw)) + Cfg::TAB_OFF);
+        for (uint32_t i = threadIdx.x; i < 1024u * REP; i += blockDim.x)
+            tab[i] = __ldg(crc_tab + i / REP);
+    }
     if (threadIdx.x == 0) {
         for (int s = 0; s < (int)STAGES; ++s) {
             mbar_init(bar_full + s * 8, 1);
@@ -424,6 +513,7 @@ k_roll_scan(const __grid_constant__ CUtensorMap tm_main, uint32_t n_tiles, uint3
     const uint32_t row = wt * 32u + lane;   // row of the tile; it sits at box row `row + 1`, the row above it at `row`
     const uint32_t ra_off = (row + 1u) * 128u, swz = ((row + 1u) & 7u) << 4;
     const uint32_t rp_off = row * 128u, swp = (row & 7u) << 4;
+    const uint32_t T = s0 + Cfg::TAB_OFF + (REP > 0 ? lane % REP : 0u) * 4u; // this lane's table copy
     uint32_t blk_next = 0, blk_end = 0; // this warp's private slice of the pool (warp-uniform)
     // CTA-local tile sequence it = 0,1,2,... (global tile = blockIdx.x + it*gridDim.x); group g takes it = g (mod GROUPS)
     for (uint32_t it = group;; it += SCAN_GROUPS) {
@@ -451,9 +541,16 @@ k_roll_scan(const __grid_constant__ CUtensorMap tm_main, uint32_t n_tiles, uint3
         const uint32_t ra = sb + ra_off;
         uint32_t mL0 = 0, mL1 = 0, mL2 = 0, mL3 = 0; // loose candidates, bit p of the row
         uint32_t mS0 = 0, mS1 = 0, mS2 = 0, mS3 = 0; // strict candidates
+        uint32_t hc = 0;                             // CRC chain of the row (REP > 0)
 #pragma unroll
         for (int c = 0; c < 8; ++c) {
             const uint4 w = lds_u128(ra + ((uint32_t)(c << 4) ^ swz));
+            if constexpr (REP > 0) {
+                hc = c == 0 ? w.x : crc_step_rep<REP>(T, hc, w.x);
+                hc = crc_step_rep<REP>(T, hc, w.y);
+                hc = crc_step_rep<REP>(T, hc, w.z);
+                hc = crc_step_rep<REP>(T, hc, w.w);
+            }
             uint32_t hv[16];
             MK_ROLL_WORD(pw, w.x, 0) MK_ROLL_WORD(w.x, w.y, 4) MK_ROLL_WORD(w.y, w.z, 8) MK_ROLL_WORD(w.z, w.w, 12)
             pw = w.w;
@@ -486,6 +583,8 @@ k_roll_scan(const __grid_constant__ CUtensorMap tm_main, uint32_t n_tiles, uint3
         __syncwarp();
         if (lane == 0)
             mbar_arrive(bar_empty + s * 8);
+        if constexpr (REP > 0)
+            part[(size_t)tile * Cfg::ROWS + row] = hc;
 
         // ordered compaction: lane l's candidates precede lane l+1's
         const uint32_t cnt = __popc(mL0) + __popc(mL1) + __popc(mL2) + __popc(mL3);
