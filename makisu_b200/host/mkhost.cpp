@@ -315,17 +315,11 @@ size_t mkhost_memfs_describe_update_from_tar_ex(mkhost_memfs *m, int64_t now_uni
         m->fs.set_now(now_unix);
         std::vector<uint8_t> buf;
         uint8_t tmp[65536];
-        for (;;) {
-            ssize_t r = read(tar_fd, tmp, sizeof tmp);
-            if (r < 0) {
-                if (errno == EINTR)
-                    continue;
-                throw HostError(std::string("read header: ") + strerror(errno));
-            }
-            if (r == 0)
-                break;
+        uint64_t r;
+        do {
+            r = read_full(tar_fd, tmp, sizeof tmp, "read header");
             buf.insert(buf.end(), tmp, tmp + r);
-        }
+        } while (r == sizeof tmp);
         MemTarSource src(buf.data(), buf.size());
         if (flags & MKHOST_UNTAR) {
             MemFS::Untar u;
@@ -360,18 +354,12 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
         const std::vector<TarMember> members =
             untar ? read_tar(src, [&](const TarMember &mem, const uint8_t *body) { m->fs.untar_member(u, mem, body); }) // files written from the arena
                   : read_tar(src);
-        src.flush(true);
+        src.s.submit_tar(true);
         mksnap_result res;
-        ck(eng, mksnap_finish(eng, &res), "finish");
-        memset(out->tar_digest, 0, 32);
-        std::vector<uint8_t> d((size_t)(src.n_file_streams + 1) * 32);
-        if (want_digest || src.n_file_streams)
-            ck(eng, mksnap_get_stream_digests(eng, d.data(), src.n_file_streams + 1), "stream digests");
-        if (want_digest)
-            memcpy(out->tar_digest, d.data(), 32);
-        memcpy(out->root, res.root, 32);
+        const uint32_t n_files = src.s.n_file_streams;
+        const std::vector<uint8_t> d = src.s.finish(res, n_files + 1, want_digest || n_files);
         const std::map<std::string, MemFile> layer = untar ? m->fs.untar_finish(u) : m->fs.update_from_tar(members);
-        out->n_entries = layer.size();
+        set_layer_result(out, res, want_digest ? d.data() : nullptr, layer.size(), src.s.tar_bytes);
         if (file_digests) { // remember the content digest of every regular member that made it into the tree
             uint32_t k = 0;
             for (const auto &mem : members) {
@@ -384,9 +372,6 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
                     m->fs.set_digest(dst, d.data() + 32 * k);
             }
         }
-        out->tar_bytes = src.tar_bytes;
-        out->n_chunks = res.n_chunks;
-        out->n_unique = res.n_unique;
         return 0;
     } catch (const std::exception &e) {
         set_err(err, errlen, std::string("update memfs from tar: ") + e.what());
@@ -475,33 +460,23 @@ static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc
         uint64_t total = prefix_len;
         for (const auto &g : segs)
             total += g.kind == 'F' ? g.size : g.bytes.size();
-        ck(eng, mksnap_begin(eng), "begin");
-
-        const mksnap_limits lim = engine_limits(eng);
-        void *hp = nullptr;
-        uint64_t cap = 0;
-        ArenaLease lease(eng);
-        int32_t &aid = lease.id;
-        uint64_t pos = 0;
-        std::vector<mksnap_extent> ext;
-        std::vector<ReadJob> jobs;
-        auto acquire = [&]() {
-            const auto t = std::chrono::steady_clock::now();
-            ck(eng, mksnap_arena_acquire(eng, &hp, &cap, &aid), "arena acquire");
-            ms_acquire += ms_since(t);
-            pos = 0;
-            ext.clear();
-            jobs.clear();
-        };
-        auto flush = [&]() {
-            auto t = std::chrono::steady_clock::now();
-            run_reads(jobs, n_threads);
+        ArenaSession s(eng, n_threads, 1); // cap unrounded: CRC pieces end anywhere, files are cut at 16-byte granularity
+        auto t = std::chrono::steady_clock::now();
+        s.after_reads = [&]() {
             ms_reads += ms_since(t);
             t = std::chrono::steady_clock::now();
-            ck(eng, mksnap_arena_submit(eng, aid, pos, ext.data(), ext.size(), nullptr, 0), "arena submit");
-            ms_submit += ms_since(t);
-            aid = -1;
         };
+        auto acquire = [&]() {
+            t = std::chrono::steady_clock::now();
+            s.acquire();
+            ms_acquire += ms_since(t);
+        };
+        auto flush = [&]() {
+            t = std::chrono::steady_clock::now();
+            s.submit();
+            ms_submit += ms_since(t);
+        };
+        ck(eng, mksnap_begin(eng), "begin");
         acquire();
         uint64_t after = total; // stream bytes not yet placed
         uint64_t n_crc_ext = 0; // CRC extents submitted so far in this session (index into mksnap_get_extent_crcs)
@@ -515,20 +490,19 @@ static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc
         auto put_bytes = [&](const void *p, size_t n) {
             if (n == 0)
                 return;
-            uint64_t o = align_up(pos, 16);
-            if (o + n > cap || ext.size() >= lim.max_extents) { // the extent table fills before the arena on tiny files
-
+            uint64_t o = align_up(s.pos, 16);
+            if (o + n > s.cap || !s.room(1, 0)) {
                 flush();
                 acquire();
                 o = 0;
             }
-            if (n > cap)
+            if (n > s.cap)
                 throw HostError("path string larger than the arena");
-            memcpy((uint8_t *)hp + o, p, n);
+            memcpy(s.a + o, p, n);
             after -= n;
-            ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
+            s.ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
             ++n_crc_ext;
-            pos = o + n;
+            s.pos = o + n;
         };
         put_bytes(prefix, prefix_len);
         for (const auto &g : segs) {
@@ -553,20 +527,20 @@ static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc
                 sent.push_back(Sent{&g, n_crc_ext, {}});
             uint64_t done = 0; // CRC is linear: a file may be split across arenas at any 16-byte boundary
             while (done < g.size) {
-                uint64_t o = align_up(pos, 512);
-                if (o + 4096 > cap || ext.size() >= lim.max_extents) {
+                uint64_t o = align_up(s.pos, 512);
+                if (o + 4096 > s.cap || !s.room(1, 0)) {
                     flush();
                     acquire();
                     o = 0;
                 }
-                uint64_t n = std::min<uint64_t>(g.size - done, (cap - o) / 16 * 16);
-                jobs.push_back(ReadJob{g.path, done, n, (uint8_t *)hp + o});
+                uint64_t n = std::min<uint64_t>(g.size - done, (s.cap - o) / 16 * 16);
+                s.jobs.push_back(ReadJob{g.path, done, n, s.a + o});
                 after -= n;
-                ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
+                s.ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
                 ++n_crc_ext;
                 if (cache)
                     sent.back().piece_len.push_back(n);
-                pos = o + n;
+                s.pos = o + n;
                 done += n;
             }
         }

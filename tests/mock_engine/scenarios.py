@@ -363,7 +363,7 @@ def random_trees_small_arenas(make_engine, tmp):
 def table_limits_and_arena_leases(make_engine, tmp):
     """ADVICE round 1: (a) a context of many tiny files fills max_extents long before it fills an arena -- the packers
     flush early instead of failing with E_CAPACITY (the reference handles any file count, add_copy_step.go:153-169);
-    (b) a packer that throws between acquire and submit gives its arena back (ArenaLease): the handle survives more
+    (b) a packer that throws between acquire and submit gives its arena back (ArenaSession): the handle survives more
     failures than it has arenas."""
     ctx = os.path.join(tmp, "tiny")
     rng = np.random.default_rng(11)
