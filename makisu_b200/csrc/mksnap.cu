@@ -979,15 +979,11 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
             order = h->d_order;
         }
         if (h->sha_fma)
-            k_sha256_ranges<true><<<sha_grid(h), SHA_THREADS, 0, sk>>>(d_arena, h->d_chunk_start, h->d_chunk_len,
-                                                                      &h->d_sc->batch_chunks, 0, &h->d_sc->n_chunks, 0, 0,
-                                                                      0, h->d_digests, &h->d_sc->work, &h->d_sc->err, 1u, nullptr, nullptr,
-                                                                      nullptr, order);
+            k_sha256_ranges<true><<<sha_grid(h), SHA_THREADS, 0, sk>>>(d_arena, h->d_chunk_start, h->d_chunk_len, h->d_sc,
+                                                                      h->d_digests, 1u, order);
         else
-            k_sha256_ranges<false><<<sha_grid(h), SHA_THREADS, 0, sk>>>(d_arena, h->d_chunk_start, h->d_chunk_len,
-                                                                       &h->d_sc->batch_chunks, 0, &h->d_sc->n_chunks, 0,
-                                                                       0, 0, h->d_digests, &h->d_sc->work, &h->d_sc->err, 1u, nullptr, nullptr,
-                                                                      nullptr, order);
+            k_sha256_ranges<false><<<sha_grid(h), SHA_THREADS, 0, sk>>>(d_arena, h->d_chunk_start, h->d_chunk_len, h->d_sc,
+                                                                       h->d_digests, 1u, order);
         LAUNCH_OK(h);
         k_batch_end<<<1, 32, 0, sk>>>(h->d_sc);
         LAUNCH_OK(h);

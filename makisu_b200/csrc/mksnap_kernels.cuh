@@ -3,9 +3,9 @@
 //   K0  k_crc32_extents   CRC-32/IEEE of the context stream      (HBM-read bound, or a combine of K1's row CRCs)
 //   K1  k_roll_scan       Roll-32 candidate scan [+ row CRCs]    (HBM-read bound)
 //   K1b k_select_cuts     min/normal/max cut selection per file  (latency, tiny)
-//   K2  k_sha256_ranges   SHA-256 of many byte ranges            (int-ALU bound)
-//       (the same kernel digests the serial layer-tar streams, K4, and the
-//        Merkle levels of the table root)
+//   K2  k_sha256_ranges   SHA-256 of the chunks                  (int-ALU bound)
+//       (the serial layer-tar streams and the Merkle levels of the table root
+//        are K4, mksnap_sha_stream.cuh)
 //   K3  radix sort / unique of 256-bit digests                   (HBM, tiny)
 //
 // Reference arithmetic being replaced (all Go stdlib behind these call sites):
@@ -1178,18 +1178,20 @@ __global__ void __launch_bounds__(LEN_THREADS) k_len_order(const uint64_t *__res
 }
 
 // ------------------------------------------------------------------------
-// K2 / K4: SHA-256 of byte ranges.  One lane per range, one 64-byte block per
-// loop iteration; a lane that finishes its range pulls the next one from a
-// global counter, so a warp stays converged on "compress one block" no matter
-// how ragged the range lengths are.  Ranges start at arbitrary byte
-// alignment (cut points are content defined): five aligned 16-byte loads
-// cover the block, two select stages rotate by words and one PRMT per word
+// K2: SHA-256 of the chunks of the chunk table.  One lane per chunk, one
+// 64-byte block per loop iteration; a lane that finishes its chunk pulls the
+// next one from a global counter, so a warp stays converged on "compress one
+// block" no matter how ragged the chunk lengths are.  Chunks start at
+// arbitrary byte alignment (cut points are content defined): each lane
+// stages the five aligned 16-byte words that cover its block in shared
+// memory and reads the 17 words from the one that holds the block's first
+// byte back, so the word rotation costs no ALU instruction; one PRMT per word
 // does the byte shift and the big-endian swap together.
 // ------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t rotr(uint32_t x, int n) { return __funnelshift_r(x, x, n); }
 
 // FMA_ADDS = true: additions as IMAD (throughput: many chunks, ALU pipe saturated);
-// false: plain adds (IADD3, shorter dependent chain) for the latency-bound serial streams.
+// false: plain adds (IADD3, shorter dependent chain).
 template <bool FMA_ADDS> __device__ __forceinline__ uint32_t sha_add(uint32_t a, uint32_t b, uint32_t one)
 {
     return FMA_ADDS ? fma_add_rt(a, b, one) : a + b;
@@ -1266,140 +1268,148 @@ __device__ __forceinline__ void sha256_compress(uint32_t st[8], uint32_t w[16], 
 }
 
 constexpr int SHA_THREADS = 128;
+constexpr int SHA_WIN = 5; // 16-byte words of a block's aligned window: 80 bytes cover 64 at any alignment
 
-// StreamState (midstate of a serial stream that continues in a later submit): mksnap_sha_stream.cuh
+// Stage a block's window (SHA_WIN aligned 16-byte words from q; word k only if bit k of `mask` is set) at shared
+// address `wr`.
+__device__ __forceinline__ void sha_stage(uint32_t wr, const uint4 *q, uint32_t mask)
+{
+#pragma unroll
+    for (int k = 0; k < SHA_WIN; ++k)
+        if (mask & (1u << k)) {
+            const uint4 v = __ldg(q + k);
+            asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};"
+                         :: "r"(wr + 16 * k), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w));
+        }
+}
 
-// mode 0: ranges from (start[], len[]) arrays, count read from *n_dev (or n_host if n_dev==nullptr)
-// mode 1: uniform ranges of `uni_len` bytes over [0, uni_total) of `data` (Merkle levels)
+// The 16 big-endian message words of a staged block: 17 words from shared address `rd` (the word holding the block's
+// first byte), one PRMT each for the byte shift and the swap.
+__device__ __forceinline__ void sha_unstage(uint32_t w[16], uint32_t rd, uint32_t sel)
+{
+    uint32_t z[17];
+#pragma unroll
+    for (int i = 0; i < 17; ++i)
+        asm volatile("ld.shared.u32 %0, [%1];" : "=r"(z[i]) : "r"(rd + 4 * i));
+#pragma unroll
+    for (int i = 0; i < 16; ++i) // prmt, not __byte_perm: `sel` is a valid selector, no mask per block
+        asm("prmt.b32 %0, %1, %2, %3;" : "=r"(w[i]) : "r"(z[i]), "r"(z[i + 1]), "r"(sel));
+}
+
+// Chunk i of the batch is row sc->n_chunks + i of start/len/out; `order` (or nullptr: batch order) is the order in
+// which the lanes take them.  A chunk is at most max_size (32-bit) bytes long.
 template <bool FMA_ADDS>
 __global__ void SHA_LAUNCH_BOUNDS
-k_sha256_ranges(const uint8_t *__restrict__ data, const uint64_t *__restrict__ start,
-                const uint64_t *__restrict__ len, const uint32_t *__restrict__ n_dev, uint64_t n_host,
-                const unsigned long long *__restrict__ first_dev, uint64_t first_host, /* index of range 0 in start/len/out */
-                uint64_t uni_len, uint64_t uni_total, uint8_t *__restrict__ out,
-                uint32_t *__restrict__ work_counter, const uint32_t *__restrict__ skip_if_err, const uint32_t one,
-                const uint32_t *__restrict__ rng_stream, const uint32_t *__restrict__ rng_flags,
-                StreamState *__restrict__ sstate, const uint32_t *__restrict__ order /* work order or nullptr */)
+k_sha256_ranges(const uint8_t *__restrict__ data, const uint64_t *__restrict__ start, const uint64_t *__restrict__ len,
+                SessionCounters *__restrict__ sc, uint8_t *__restrict__ out, const uint32_t one,
+                const uint32_t *__restrict__ order)
 {
-    if (skip_if_err && *skip_if_err)
+    // a lane's window at a stride of 20 words: the STS.128 of a quarter warp hit 8 distinct 16-byte bank groups
+    __shared__ uint4 s_win[SHA_THREADS * SHA_WIN];
+    if (sc->err)
         return;
-    const uint64_t n = n_dev ? (uint64_t)*n_dev : n_host;
-    const uint64_t first = first_dev ? (uint64_t)*first_dev : first_host;
+    const uint32_t n = sc->batch_chunks;
+    const uint64_t first = sc->n_chunks;
     const uint32_t lane = threadIdx.x & 31;
+    const uint32_t base = (uint32_t)__cvta_generic_to_shared(s_win + threadIdx.x * SHA_WIN);
 
     uint32_t st[8];
-    const uint8_t *p = nullptr; // next block to read
-    uint64_t total = 0;         // range length
-    uint64_t done = 0;          // bytes already compressed
-    uint64_t my = 0;            // range index (row of `out`; the stream slot in stream mode)
-    uint64_t prior = 0;         // bytes of this stream compressed in earlier pieces
-    bool more = false;          // this piece is not the last of its stream
-    uint32_t phase = 0;         // 0 idle, 1 data blocks, 2 needs extra length block
+    const uint4 *q = nullptr; // window of the next block: its first 16-byte word holds the block's first byte
+    uint32_t a = 0;           // the chunk's start mod 16, the same for every block of it
+    uint32_t wr = base;       // shared address of this lane's window
+    uint32_t rd = 0;          // shared address of the window's word that holds the block's first byte
+    uint32_t sel = 0;         // PRMT selector: byte shift by a & 3 and big-endian swap
+    uint32_t left = 0;        // phase 1: bytes of the chunk not yet compressed; otherwise 0
+    uint32_t total = 0;       // chunk length
+    uint64_t my = 0;          // row of the chunk in start/len/out
+    uint32_t phase = 0;       // 0 idle, 1 data blocks, 2 needs extra length block
     bool exhausted = false;
 
     for (;;) {
-        // ---- refill idle lanes (warp-aggregated fetch) ----
-        const uint32_t need = __ballot_sync(0xFFFFFFFFu, phase == 0 && !exhausted);
-        if (need) {
-            uint32_t basei = 0;
-            const uint32_t leader = __ffs(need) - 1;
-            if (lane == leader)
-                basei = atomicAdd(work_counter, __popc(need));
-            basei = __shfl_sync(0xFFFFFFFFu, basei, leader);
-            if (phase == 0 && !exhausted) {
-                const uint64_t idx = (uint64_t)basei + __popc(need & ((1u << lane) - 1u));
-                if (idx < n) {
-                    my = first + (order ? (uint64_t)order[idx] : idx);
-                    if (start) {
-                        p = data + start[my];
-                        total = len[my];
+        // Only a lane within 80 bytes of its chunk's end, or without a chunk, needs more than a full block.
+        bool full = __all_sync(0xFFFFFFFFu, left >= 80);
+        if (!full) {
+            // ---- refill idle lanes (warp-aggregated fetch) ----
+            const uint32_t need = __ballot_sync(0xFFFFFFFFu, phase == 0 && !exhausted);
+            if (need) {
+                uint32_t basei = 0;
+                const uint32_t leader = __ffs(need) - 1;
+                if (lane == leader)
+                    basei = atomicAdd(&sc->work, __popc(need));
+                basei = __shfl_sync(0xFFFFFFFFu, basei, leader);
+                if (phase == 0 && !exhausted) {
+                    const uint32_t idx = basei + __popc(need & ((1u << lane) - 1u));
+                    if (idx < n) {
+                        my = first + (order ? order[idx] : idx);
+                        const uint8_t *p = data + start[my];
+                        total = left = (uint32_t)len[my];
+                        a = (uint32_t)((uintptr_t)p & 15u);
+                        q = reinterpret_cast<const uint4 *>(p - a);
+                        rd = base + (a & 12u);
+                        wr = rd & ~15u; // = base; derived from rd so that it stays in a register
+                        sel = 0x0123u + 0x1111u * (a & 3u);
+                        phase = 1;
+                        st[0] = 0x6a09e667; st[1] = 0xbb67ae85; st[2] = 0x3c6ef372; st[3] = 0xa54ff53a;
+                        st[4] = 0x510e527f; st[5] = 0x9b05688c; st[6] = 0x1f83d9ab; st[7] = 0x5be0cd19;
                     } else {
-                        const uint64_t o = idx * uni_len;
-                        p = data + o;
-                        total = uni_total - o < uni_len ? uni_total - o : uni_len;
+                        exhausted = true;
                     }
-                    done = 0;
-                    phase = 1;
-                    prior = 0;
-                    more = false;
-                    st[0] = 0x6a09e667; st[1] = 0xbb67ae85; st[2] = 0x3c6ef372; st[3] = 0xa54ff53a;
-                    st[4] = 0x510e527f; st[5] = 0x9b05688c; st[6] = 0x1f83d9ab; st[7] = 0x5be0cd19;
-                    if (rng_stream) { // serial stream piece: resume the saved midstate, digest row = stream slot
-                        const uint32_t sid = rng_stream[my];
-                        more = (rng_flags[my] & 1u) != 0;
-                        my = sid;
-                        if (sstate[sid].open) {
-#pragma unroll
-                            for (int k = 0; k < 8; ++k)
-                                st[k] = sstate[sid].st[k];
-                            prior = sstate[sid].bytes;
-                        }
-                    }
-                } else {
-                    exhausted = true;
                 }
             }
+            if (!__any_sync(0xFFFFFFFFu, phase != 0))
+                break;
+            full = left >= 80;
         }
-        if (!__any_sync(0xFFFFFFFFu, phase != 0))
-            break;
-        if (phase == 0)
-            continue;
 
         uint32_t w[16];
-        const uint64_t rem = total - done;
         bool last = false;
-        if (phase == 2) {
+        if (full) {
+            // full block: the window starts at or before the block and ends before its byte 80, inside the chunk
+            sha_stage(wr, q, 0x1Fu);
+            sha_unstage(w, rd, sel);
+            q += 4;
+            left -= 64;
+        } else if (phase == 0) {
+            continue;
+        } else if (phase == 2) {
 #pragma unroll
             for (int i = 0; i < 14; ++i)
                 w[i] = 0;
-            w[14] = (uint32_t)(((prior + total) * 8) >> 32);
-            w[15] = (uint32_t)((prior + total) * 8);
+            w[14] = total >> 29;
+            w[15] = total << 3;
             last = true;
         } else {
-            // aligned 80-byte window covering [p, p+64); only 16-byte words that intersect [p, p+min(rem,64)) are
-            // touched.  (Fetching the next block's window ahead of the compress was measured slower.)
-            const uint32_t a = (uint32_t)((uintptr_t)p & 15u);
-            const uint4 *q = reinterpret_cast<const uint4 *>(p - a);
-            const uint32_t lim = a + (rem < 64 ? (uint32_t)rem : 64u);
-            uint32_t x[20];
+            // the chunk's last one or two blocks: only the 16-byte words that hold bytes of the chunk are read.  The
+            // others keep an earlier block's bytes, which all lie past the chunk's end and are masked off below.
+            const uint32_t lim = a + (left < 64 ? left : 64u);
+            uint32_t mask = 0;
 #pragma unroll
-            for (int k = 0; k < 5; ++k) {
-                uint4 v = make_uint4(0, 0, 0, 0);
-                if ((uint32_t)(16 * k) < lim)
-                    v = __ldg(q + k);
-                x[4 * k] = v.x; x[4 * k + 1] = v.y; x[4 * k + 2] = v.z; x[4 * k + 3] = v.w;
-            }
-            uint32_t y[18];
-#pragma unroll
-            for (int i = 0; i < 18; ++i)
-                y[i] = (a & 8u) ? x[i + 2] : x[i];
-            uint32_t z[17];
-#pragma unroll
-            for (int i = 0; i < 17; ++i)
-                z[i] = (a & 4u) ? y[i + 1] : y[i];
-            const uint32_t sel = 0x0123u + 0x1111u * (a & 3u);
-#pragma unroll
-            for (int i = 0; i < 16; ++i)
-                w[i] = __byte_perm(z[i], z[i + 1], sel);
-            if (rem < 64) {
-                // final data block: keep `rem` bytes, append 0x80, zero the rest
-                const uint32_t rb = (uint32_t)rem;
+            for (int k = 0; k < SHA_WIN; ++k)
+                mask |= (uint32_t)(16 * k < lim) << k;
+            sha_stage(wr, q, mask);
+            sha_unstage(w, rd, sel);
+            if (left >= 64) {
+                q += 4;
+                left -= 64;
+            } else {
+                // final data block: keep `left` bytes, append 0x80, zero the rest
 #pragma unroll
                 for (int i = 0; i < 16; ++i) {
-                    const int32_t k = (int32_t)rb - 4 * i; // valid bytes in this word
+                    const int32_t k = (int32_t)left - 4 * i; // valid bytes in this word
                     uint32_t keep = k >= 4 ? 0xFFFFFFFFu : (k <= 0 ? 0u : ~(0xFFFFFFFFu >> (8 * k)));
                     uint32_t v = w[i] & keep;
                     if (k >= 0 && k < 4)
                         v |= 0x80000000u >> (8 * k);
                     w[i] = v;
                 }
-                if (rb < 56) {
-                    w[14] = (uint32_t)(((prior + total) * 8) >> 32);
-                    w[15] = (uint32_t)((prior + total) * 8);
+                if (left < 56) {
+                    w[14] = total >> 29;
+                    w[15] = total << 3;
                     last = true;
                 } else {
                     phase = 2;
                 }
+                left = 0;
             }
         }
         sha256_compress<FMA_ADDS>(st, w, one);
@@ -1412,20 +1422,7 @@ k_sha256_ranges(const uint8_t *__restrict__ data, const uint64_t *__restrict__ s
             uint4 *dst = reinterpret_cast<uint4 *>(out + my * 32);
             dst[0] = o0;
             dst[1] = o1;
-            if (rng_stream)
-                sstate[my].open = 0;
             phase = 0;
-        } else if (phase == 1) {
-            p += 64;
-            done += 64;
-            if (more && done == total) { // piece boundary (length is a multiple of 64): park the midstate
-#pragma unroll
-                for (int k = 0; k < 8; ++k)
-                    sstate[my].st[k] = st[k];
-                sstate[my].bytes = prior + total;
-                sstate[my].open = 1;
-                phase = 0;
-            }
         }
     }
 }
