@@ -93,6 +93,41 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
                                 uint32_t *crc_out, uint64_t *stream_len_out, mkhost_crc_cache_stats *stats, char *err,
                                 size_t errlen);
 
+/* cacheID of every step of a build plan (processStagesAndAliases + createDockerfileSteps, lib/builder/build_plan.go:93-160,
+ * build_stage.go:153-165: each step is seeded with the cacheID of the step before it), with the context read once for
+ * the whole plan.  The sources of every COPY/ADD step are walked like mkhost_context_crc32 walks them; a file that
+ * several steps cover (same path, device, inode, size, mtime and ctime) travels to the device once, and so does each
+ * distinct path string and link target.  The device then folds every step's stream out of those values (mksnap_crc_fold)
+ * and the host prepends seed + directive + args step by step (mksnap_crc_prepend).  ids_out[i] is what
+ * checksum.Sum32() returns for step i; "%x" of it is the step's cacheID and the next step's seed.  A plan with more
+ * COPY/ADD steps than the engine has stream slots runs as consecutive sessions; a file read in one is not read again.
+ * With a cache, files it vouches for are not read at all and every file that travelled is remembered, like
+ * mkhost_context_crc32_cached.  stats: files_total / bytes_total count every occurrence over all steps, files_reused
+ * the occurrences folded from the cache, bytes_sent each file that travelled once.  Steps come in plan order, the
+ * stages in order, with the stage of a remote image that a COPY --from names (build_plan.go:142-152) in front of the
+ * stage that names it. */
+#define MKHOST_STEP_COPY 1        /* addCopyStep.SetCacheID (add_copy_step.go:102-122): directive "COPY"/"ADD"; a
+                                     non-empty from_stage (COPY --from) hashes no content (add_copy_step.go:109-113) */
+#define MKHOST_STEP_FROM 2        /* FromStep.SetCacheID: crc32(seed + "FROM" + args), args = image (from_step.go:79-83) */
+#define MKHOST_STEP_BASE 3        /* baseStep.SetCacheID: crc32(seed + directive + args + "true"/"false" of commit)
+                                     (base_step.go:62-67): RUN, ENV, CMD, ... */
+#define MKHOST_STEP_REMOTE_FROM 4 /* the FROM step of a remote-image stage (newRemoteImageStage, build_stage.go:78-108).
+                                     The stage that names the image was seeded before it was inserted: a run of these
+                                     chains from the seed of the step in front of them, and the step after the run takes
+                                     that same seed again. */
+typedef struct {
+    uint32_t kind;
+    int32_t commit;             /* MKHOST_STEP_BASE */
+    const char *directive;      /* COPY / BASE */
+    const char *args;           /* as the reference prints them; the image of a FROM */
+    const char *from_stage;     /* COPY: NULL or "" = sources from the context */
+    const char *const *from_paths;
+    size_t n_paths;
+} mkhost_plan_step;
+int mkhost_plan_cache_ids(mksnap_t *eng, mkhost_crc_cache *cache, const char *seed, const char *context_dir,
+                          const mkhost_plan_step *steps, size_t n_steps, int n_threads, uint32_t *ids_out,
+                          mkhost_crc_cache_stats *stats, char *err, size_t errlen);
+
 /* Commit one layer from copy operations against an EMPTY MemFS rooted at root_dir (FROM scratch): packs
  * the sorted entries as a tar stream into one arena, digests it (TarDigest) and chunks every regular
  * file (chunk table).  now_unix = clk.Now() for synthesized ancestors (mem_fs.go:562). */

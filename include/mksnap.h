@@ -218,6 +218,29 @@ int mksnap_crc_add(mksnap_t *h, uint32_t pure, uint64_t len, uint64_t crc_suffix
 uint32_t mksnap_crc_concat(uint32_t pure_a, uint32_t pure_b, uint64_t len_b);
 int mksnap_get_extent_crcs(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint64_t *n_out);
 
+/* ---- plan-level cacheIDs: many CRC streams from one session's extent values ----
+ * Every COPY/ADD step of a build plan hashes its own stream (add_copy_step.go:102-122), and the steps share segments:
+ * `COPY requirements.txt .` then `COPY . .`.  Each unique segment travels once as a MKSNAP_X_CRC extent; then
+ * mksnap_crc_fold XORs, per use, value * x^(8 * suffix) into stream slot `stream` of this session on the device
+ * (k_crc_fold), where suffix = bytes of that stream after the use.  The value is pure(extent) of the CRC extent `src`
+ * (mksnap_get_extent_crcs numbering; it must already be submitted) or, with MKSNAP_U_VALUE, the low 32 bits of src (a
+ * value the caller remembered).  Stream slots are [0, max_streams) and start at zero in every session.  Call between
+ * begin and finish, at most max_extents uses per call; `uses` may be reused when the call returns.  A session whose CRC
+ * extents outran the engine's per-extent table fails the fold (MKSNAP_E_CAPACITY) rather than fold a value it did not
+ * keep.  The prefix seed + directive + args is not part of a stream: mksnap_crc_prepend adds it on the host. */
+#define MKSNAP_U_VALUE 1u
+typedef struct {
+    uint64_t suffix;
+    uint64_t src;
+    uint32_t stream;
+    uint32_t flags;
+} mksnap_crc_use;
+int mksnap_crc_fold(mksnap_t *h, const mksnap_crc_use *uses, uint64_t n);
+/* after finish: pure value of the streams [0, *n_out), n_out = highest stream slot folded + 1 */
+int mksnap_get_crc_streams(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint64_t *n_out);
+/* host arithmetic, no device: checksum.Sum32() of prefix || rest, given pure(rest) and len(rest) */
+uint32_t mksnap_crc_prepend(const void *prefix, uint64_t n, uint32_t pure_rest, uint64_t len_rest);
+
 /* ---- result tables (valid after mksnap_finish, until the next begin) ---- */
 /* chunk END offsets (exclusive; position in the concatenation of all submitted
  * arenas) and digests, in (submit, extent, position) order. */

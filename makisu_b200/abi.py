@@ -51,6 +51,13 @@ class Range(C.Structure):
 MKSNAP_R_MORE = 1
 
 
+class CrcUse(C.Structure):
+    _fields_ = [("suffix", C.c_uint64), ("src", C.c_uint64), ("stream", C.c_uint32), ("flags", C.c_uint32)]
+
+
+MKSNAP_U_VALUE = 1  # CrcUse.src holds the pure value itself, not an extent index
+
+
 class Result(C.Structure):
     _fields_ = [("crc_pure", C.c_uint32), ("reserved", C.c_uint32), ("crc_bytes", C.c_uint64),
                 ("cdc_bytes", C.c_uint64), ("n_files", C.c_uint64), ("n_chunks", C.c_uint64),
@@ -90,6 +97,9 @@ SYMBOLS = [
     ("mksnap_crc_add", C.c_int, [_P, C.c_uint32, C.c_uint64, C.c_uint64]),
     ("mksnap_crc_concat", C.c_uint32, [C.c_uint32, C.c_uint32, C.c_uint64]),
     ("mksnap_get_extent_crcs", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("mksnap_crc_fold", C.c_int, [_P, C.POINTER(CrcUse), C.c_uint64]),
+    ("mksnap_get_crc_streams", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("mksnap_crc_prepend", C.c_uint32, [C.c_char_p, C.c_uint64, C.c_uint32, C.c_uint64]),
     ("mksnap_get_chunks", C.c_int, [_P, _P, _P, C.c_uint64]),
     ("mksnap_get_table", C.c_int, [_P, _P, C.c_uint64]),
     ("mksnap_get_stream_digests", C.c_int, [_P, _P, C.c_uint64]),
@@ -203,6 +213,20 @@ class Engine:
         self.lib.mksnap_get_extent_crcs(self.h, None, 0, C.byref(n))
         out = np.empty(max(1, n.value), dtype=np.uint32)
         self._ck(self.lib.mksnap_get_extent_crcs(self.h, out.ctypes.data, out.size, C.byref(n)), "mksnap_get_extent_crcs")
+        return out[:n.value]
+
+    def crc_fold(self, uses):
+        """uses: a ctypes array of CrcUse, or a list of (suffix, src, stream, flags) tuples."""
+        n = len(uses)
+        arr = uses if isinstance(uses, C.Array) else (CrcUse * max(1, n))(*[CrcUse(*u) for u in uses])
+        self._ck(self.lib.mksnap_crc_fold(self.h, arr, n), "mksnap_crc_fold")
+
+    def get_crc_streams(self):
+        import numpy as np
+        n = C.c_uint64()
+        self.lib.mksnap_get_crc_streams(self.h, None, 0, C.byref(n))
+        out = np.empty(max(1, n.value), dtype=np.uint32)
+        self._ck(self.lib.mksnap_get_crc_streams(self.h, out.ctypes.data, out.size, C.byref(n)), "mksnap_get_crc_streams")
         return out[:n.value]
 
     def arena_release(self, arena_id: int):
@@ -330,6 +354,11 @@ def exchange_plan(rows_per_rank, rank: int) -> dict:
     if rc:
         raise MksnapError(rc, "mksnap_exchange_plan", "")
     return dict(zip(["U", "g0", "lead", "full", "tail_own", "borrowed", "groups"], [int(v) for v in out]))
+
+
+def crc_prepend(prefix: bytes, pure_rest: int, len_rest: int) -> int:
+    """mksnap_crc_prepend: checksum.Sum32() of prefix || rest from pure(rest) and len(rest) (host arithmetic only)."""
+    return int(load().mksnap_crc_prepend(prefix, len(prefix), pure_rest, len_rest))
 
 
 def roll_multiplier() -> int:

@@ -126,6 +126,9 @@ struct mksnap {
     uint64_t crc_session_cap = 0, crc_session_n = 0;
     uint32_t crc_host_acc = 0;         // contributions folded on the host (mksnap_crc_add)
     uint64_t crc_host_bytes = 0;
+    CrcUse *d_uses = nullptr;          // mksnap_crc_fold: use table (max_extents rows) and stream values (max_streams),
+    uint32_t *d_stream_pure = nullptr; //   allocated by the first fold
+    uint64_t fold_streams = 0;         // highest stream slot folded in this session + 1
     bool open_file = false;      // the last submit ended with a MKSNAP_X_MORE extent: the next must start with its continuation
     uint8_t *d_carry = nullptr;  // open chunk of that file (k_carry_out -> k_carry_in)
     uint64_t carry_cap = 0;
@@ -686,6 +689,7 @@ void mksnap_destroy(mksnap_t *h)
     cudaFree(h->d_consts); cudaFree(h->d_sc); cudaFreeHost(h->h_sc);
     cudaFree(h->d_carry);
     cudaFree(h->d_crc_session);
+    cudaFree(h->d_uses); cudaFree(h->d_stream_pure);
     cudaFree(h->d_tiles); cudaFree(h->d_part); cudaFree(h->d_pool); cudaFree(h->d_pool_count); cudaFree(h->d_counts); cudaFree(h->d_bases);
     cudaFree(h->d_scan_tmp);
     cudaFree(h->d_order); cudaFree(h->d_chunk_start); cudaFree(h->d_chunk_len); cudaFree(h->d_chunk_end); cudaFree(h->d_digests);
@@ -709,6 +713,9 @@ int mksnap_begin(mksnap_t *h)
     CK(h, cudaStreamSynchronize(h->s_comp));
     CK(h, cudaMemsetAsync(h->d_sc, 0, sizeof(SessionCounters), h->s_comp));
     CK(h, cudaMemsetAsync(h->d_stream_state, 0, h->max_streams * sizeof(StreamState), h->s_comp));
+    if (h->fold_streams) // only the slots the last session folded into are non-zero
+        CK(h, cudaMemsetAsync(h->d_stream_pure, 0, h->fold_streams * 4, h->s_comp));
+    h->fold_streams = 0;
     for (auto &a : h->arenas) // an arena acquired but never submitted (a packer that failed half way) is reclaimed here
         a.acquired = false;
     h->n_streams = 0;
@@ -1201,6 +1208,84 @@ int mksnap_get_extent_crcs(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint6
         CK(h, cudaMemcpy(pure, h->d_crc_session, h->crc_session_n * 4, cudaMemcpyDeviceToHost));
     h->stats.d2h_bytes += h->crc_session_n * 4;
     return 0;
+}
+
+static_assert(sizeof(CrcUse) == sizeof(mksnap_crc_use), "k_crc_fold reads mksnap_crc_use rows");
+
+int mksnap_crc_fold(mksnap_t *h, const mksnap_crc_use *uses, uint64_t n)
+{
+    if (!h)
+        return MKSNAP_E_INVAL;
+    if (!uses && n)
+        return fail(h, MKSNAP_E_INVAL, "crc_fold: null use table");
+    if (!h->in_session || h->finished)
+        return fail(h, MKSNAP_E_STATE, "crc_fold outside begin/finish");
+    if (n > h->cfg.max_extents)
+        return fail(h, MKSNAP_E_CAPACITY, "crc_fold: %llu uses in one call, max_extents is %llu", (unsigned long long)n,
+                    (unsigned long long)h->cfg.max_extents);
+    if (h->crc_session_n > h->crc_session_cap)
+        return fail(h, MKSNAP_E_CAPACITY, "crc_fold: the session submitted %llu CRC extents, the per-extent table keeps %llu",
+                    (unsigned long long)h->crc_session_n, (unsigned long long)h->crc_session_cap);
+    uint64_t hi = 0;
+    for (uint64_t i = 0; i < n; i++) {
+        const mksnap_crc_use &u = uses[i];
+        if (u.flags & ~MKSNAP_U_VALUE)
+            return fail(h, MKSNAP_E_INVAL, "crc_fold: use %llu has unknown flags %#x", (unsigned long long)i, u.flags);
+        if (u.stream >= h->max_streams)
+            return fail(h, MKSNAP_E_INVAL, "crc_fold: use %llu names stream %u, max_streams is %llu", (unsigned long long)i,
+                        u.stream, (unsigned long long)h->max_streams);
+        if (!(u.flags & MKSNAP_U_VALUE) && u.src >= h->crc_session_n)
+            return fail(h, MKSNAP_E_INVAL, "crc_fold: use %llu names extent %llu, the session has submitted %llu CRC extents",
+                        (unsigned long long)i, (unsigned long long)u.src, (unsigned long long)h->crc_session_n);
+        hi = std::max<uint64_t>(hi, (uint64_t)u.stream + 1);
+    }
+    if (n == 0)
+        return 0;
+    CK(h, cudaSetDevice(h->cfg.device));
+    cudaStream_t s = h->s_comp; // after the K0 runs and the d_crc_session copies the uses read
+    if (!h->d_uses) {
+        CK(h, cudaMalloc(&h->d_uses, h->cfg.max_extents * sizeof(CrcUse)));
+        CK(h, cudaMalloc(&h->d_stream_pure, h->max_streams * 4));
+        CK(h, cudaMemsetAsync(h->d_stream_pure, 0, h->max_streams * 4, s));
+    }
+    CK(h, cudaMemcpyAsync(h->d_uses, uses, n * sizeof(CrcUse), cudaMemcpyHostToDevice, s));
+    CK(h, cudaStreamSynchronize(s)); // the caller's table is free once this returns, pinned or not
+    h->stats.h2d_bytes += n * sizeof(CrcUse);
+    k_crc_fold<<<(uint32_t)((n + FOLD_THREADS - 1) / FOLD_THREADS), FOLD_THREADS, 0, s>>>(h->d_uses, (uint32_t)n, h->d_crc_session,
+                                                                                       h->d_consts, h->d_stream_pure);
+    LAUNCH_OK(h);
+    h->fold_streams = std::max(h->fold_streams, hi);
+    return 0;
+}
+
+int mksnap_get_crc_streams(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint64_t *n_out)
+{
+    if (!h || !n_out)
+        return MKSNAP_E_INVAL;
+    if (!h->finished)
+        return fail(h, MKSNAP_E_STATE, "get_crc_streams before finish");
+    CK(h, cudaSetDevice(h->cfg.device));
+    *n_out = h->fold_streams;
+    if (h->fold_streams > capacity || (!pure && h->fold_streams))
+        return fail(h, MKSNAP_E_CAPACITY, "need %llu entries", (unsigned long long)h->fold_streams);
+    if (h->fold_streams)
+        CK(h, cudaMemcpy(pure, h->d_stream_pure, h->fold_streams * 4, cudaMemcpyDeviceToHost));
+    h->stats.d2h_bytes += h->fold_streams * 4;
+    return 0;
+}
+
+uint32_t mksnap_crc_prepend(const void *prefix, uint64_t n, uint32_t pure_rest, uint64_t len_rest)
+{
+    const uint8_t *p = static_cast<const uint8_t *>(prefix);
+    uint32_t c = 0; // pure(prefix): the CRC register from 0, no final xor
+    for (uint64_t i = 0; i < n; i++) {
+        c ^= p[i];
+        for (int k = 0; k < 8; k++)
+            c = (c >> 1) ^ (MK_CRC_POLY & (0u - (c & 1u)));
+    }
+    const uint64_t M = 0xFFFFFFFFull;
+    const uint32_t pure = crc_mulmod(c, xpow_bits(((len_rest % M) * 8ull) % M)) ^ pure_rest;
+    return pure ^ crc_mulmod(0xFFFFFFFFu, xpow_bits((((n + len_rest) % M) * 8ull) % M)) ^ 0xFFFFFFFFu;
 }
 
 int mksnap_get_chunks(mksnap_t *h, uint64_t *ends, uint8_t *digests, uint64_t capacity)

@@ -1,6 +1,7 @@
 // mksnap_kernels.cuh — hand-written sm_90a kernels of the snapshot+hash path.
 //
 //   K0  k_crc32_extents   CRC-32/IEEE of the context stream      (HBM-read bound, or a combine of K1's row CRCs)
+//   K0f k_crc_fold        extent values folded into many streams (latency, small)
 //   K1  k_roll_scan       Roll-32 candidate scan [+ row CRCs]    (HBM-read bound)
 //   K1b k_select_cuts     min/normal/max cut selection per file  (latency, tiny)
 //   K2  k_sha256_ranges   SHA-256 of the chunks                  (int-ALU bound)
@@ -325,6 +326,44 @@ k_crc32_extents(const uint8_t *__restrict__ arena, const CrcExtent *__restrict__
     }
     if (lane == 0 && warp_acc)
         atomicXor(acc_out, warp_acc);
+}
+
+// ------------------------------------------------------------------------
+// K0f: fold extent values into many CRC streams (plan-level cacheIDs, mksnap_crc_fold).
+// One thread per use: its value -- pure(extent) of this session, or an immediate value -- times x^(8*suffix), XORed
+// into the use's stream.  x^E comes from the xe byte tables as in K0: one lookup per byte of E, three products.
+// Lanes of a warp that hit the same stream XOR-reduce first (the host emits uses grouped by stream), so a warp issues
+// one atomic per distinct stream.  Latency-bound and small: 24 bytes read per use.
+// ------------------------------------------------------------------------
+struct CrcUse { // layout of mksnap_crc_use
+    uint64_t suffix;
+    uint64_t src;
+    uint32_t stream;
+    uint32_t flags; // 1: src holds the value itself
+};
+
+constexpr int FOLD_THREADS = 256;
+
+__global__ void __launch_bounds__(FOLD_THREADS)
+k_crc_fold(const CrcUse *__restrict__ uses, uint32_t n, const uint32_t *__restrict__ ext_pure,
+           const CrcConsts *__restrict__ cst, uint32_t *__restrict__ stream_pure)
+{
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    uint32_t stream = 0xFFFFFFFFu, v = 0; // past the end: a stream no use can name, value 0
+    if (i < n) {
+        const CrcUse u = uses[i];
+        const uint32_t M = 0xFFFFFFFFu; // x^(2^32-1) = 1
+        const uint32_t E = (uint32_t)(((u.suffix % M) * 8ull) % M);
+        const uint32_t val = (u.flags & 1u) ? (uint32_t)u.src : __ldg(ext_pure + u.src);
+        const uint32_t f = crc_mulmod(crc_mulmod(__ldg(&cst->xe[0][E & 255u]), __ldg(&cst->xe[1][(E >> 8) & 255u])),
+                                      crc_mulmod(__ldg(&cst->xe[2][(E >> 16) & 255u]), __ldg(&cst->xe[3][E >> 24])));
+        v = crc_mulmod(val, f);
+        stream = u.stream;
+    }
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, stream);
+    const uint32_t x = __reduce_xor_sync(peers, v);
+    if (i < n && (threadIdx.x & 31u) == (uint32_t)(__ffs(peers) - 1) && x)
+        atomicXor(stream_pure + stream, x);
 }
 
 // ------------------------------------------------------------------------

@@ -39,6 +39,11 @@ class LayerResult(C.Structure):
                 ("tar_bytes", C.c_uint64), ("n_chunks", C.c_uint64), ("n_unique", C.c_uint64)]
 
 
+class _PlanStep(C.Structure):
+    _fields_ = [("kind", C.c_uint32), ("commit", C.c_int32), ("directive", C.c_char_p), ("args", C.c_char_p),
+                ("from_stage", C.c_char_p), ("from_paths", C.POINTER(C.c_char_p)), ("n_paths", C.c_size_t)]
+
+
 _P = C.c_void_p
 SYMBOLS = [
     ("mkhost_encode_tar_header", C.c_size_t, [C.POINTER(TarHeader), _P, C.c_size_t]),
@@ -52,6 +57,8 @@ SYMBOLS = [
     ("mkhost_context_crc32_cached", C.c_int, [_P, _P, _P, C.c_size_t, C.c_char_p, C.POINTER(C.c_char_p), C.c_size_t, C.c_int,
                                               C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(CrcCacheStats), C.c_char_p,
                                               C.c_size_t]),
+    ("mkhost_plan_cache_ids", C.c_int, [_P, _P, C.c_char_p, C.c_char_p, C.POINTER(_PlanStep), C.c_size_t, C.c_int,
+                                        C.POINTER(C.c_uint32), C.POINTER(CrcCacheStats), C.c_char_p, C.c_size_t]),
     ("mkhost_commit_copy_ops", C.c_int, [_P, C.c_char_p, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_int,
                                          C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
     ("mkhost_commit_copy_ops_to_fd", C.c_int, [_P, C.c_char_p, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_int, C.c_int,
@@ -190,6 +197,54 @@ def copy_step_cache_id(eng: abi.Engine, seed: str, directive: str, args: str, co
                        from_paths: Sequence[str]) -> str:
     crc, _ = context_crc32(eng, (seed + directive + args).encode(), context_dir, from_paths)
     return "%x" % crc  # add_copy_step.go:119
+
+
+MKHOST_STEP_COPY, MKHOST_STEP_FROM, MKHOST_STEP_BASE, MKHOST_STEP_REMOTE_FROM = 1, 2, 3, 4
+
+
+@dataclass
+class PlanStep:
+    """One step of a build plan for plan_cache_ids (include/mkhost.h, mkhost_plan_step).
+    kind COPY: directive "COPY"/"ADD", from_paths its sources, from_stage set for COPY --from (no content);
+    FROM / REMOTE_FROM: args = the image; BASE: any other directive, with its commit flag."""
+    kind: int
+    directive: str = ""
+    args: str = ""
+    from_paths: Sequence[str] = ()
+    from_stage: str = ""
+    commit: bool = False
+
+    @classmethod
+    def copy(cls, directive: str, args: str, from_paths: Sequence[str], from_stage: str = ""):
+        return cls(MKHOST_STEP_COPY, directive, args, list(from_paths), from_stage)
+
+    @classmethod
+    def from_image(cls, image: str, remote: bool = False):
+        return cls(MKHOST_STEP_REMOTE_FROM if remote else MKHOST_STEP_FROM, "FROM", image)
+
+    @classmethod
+    def base(cls, directive: str, args: str, commit: bool):
+        return cls(MKHOST_STEP_BASE, directive, args, commit=commit)
+
+
+def plan_cache_ids(eng: abi.Engine, seed: str, context_dir: str, steps: Sequence[PlanStep], n_threads: int = 0,
+                   cache: Optional["CrcCache"] = None):
+    """-> (cacheID of every step as "%x", stats dict): the whole plan in one pass over the context."""
+    n = len(steps)
+    arr, keep = (_PlanStep * max(1, n))(), []
+    for i, s in enumerate(steps):
+        paths = _strs(list(s.from_paths))
+        keep.append(paths)
+        arr[i].kind, arr[i].commit = s.kind, int(s.commit)
+        arr[i].directive, arr[i].args = s.directive.encode(), s.args.encode()
+        arr[i].from_stage = s.from_stage.encode()
+        arr[i].from_paths, arr[i].n_paths = paths, len(s.from_paths)
+    ids, st, err = (C.c_uint32 * max(1, n))(), CrcCacheStats(), C.create_string_buffer(1024)
+    rc = load().mkhost_plan_cache_ids(eng.h, cache.h if cache is not None else None, seed.encode(), os.fsencode(context_dir),
+                                      arr, n, n_threads, ids, C.byref(st), err, len(err))
+    if rc:
+        raise HostError(err.value.decode())
+    return ["%x" % ids[i] for i in range(n)], {k: getattr(st, k) for k, _ in CrcCacheStats._fields_}
 
 
 MKHOST_NO_TAR_DIGEST = 1

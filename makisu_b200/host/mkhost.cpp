@@ -30,6 +30,7 @@
 #include <chrono>
 #include <string>
 #include <thread>
+#include <tuple>
 #include <vector>
 
 namespace {
@@ -652,6 +653,214 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
     }
     return context_crc32_impl(eng, cache, stats, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads, crc_out,
                               stream_len_out, err, errlen);
+}
+
+// One engine session of mkhost_plan_cache_ids: the streams of the walked COPY/ADD steps `batch` (stream slot k = batch[k]).
+// Every distinct path string / link target and every file not yet valued travels once as CRC extents (crc_suffix 0:
+// only pure(extent) is wanted); each occurrence in a stream becomes a use of those extents, or of a known value.
+using FileKey = std::tuple<std::string, uint64_t, uint64_t, uint64_t, int64_t, int64_t>; // path, dev, ino, size, mtime, ctime
+static FileKey file_key(const Seg &g) { return FileKey{g.path, g.dev, g.ino, g.size, g.mtime_ns, g.ctime_ns}; }
+
+static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vector<std::vector<Seg>> &segs,
+                         const std::vector<size_t> &batch, int n_threads, std::map<FileKey, uint32_t> &known,
+                         bool remember, std::vector<uint32_t> &pure, std::vector<uint64_t> &slen,
+                         mkhost_crc_cache_stats &st, double &ms_fold)
+{
+    ArenaSession s(eng, n_threads, 1); // cap unrounded, as in the single-step pass
+    ck(eng, mksnap_begin(eng), "begin");
+    s.acquire();
+    uint64_t n_ext = 0; // CRC extents submitted so far (mksnap_get_extent_crcs numbering)
+    auto place = [&](uint64_t align, uint64_t need) {
+        uint64_t o = align_up(s.pos, align);
+        if (o + need > s.cap || !s.room(1, 0)) {
+            s.submit();
+            s.acquire();
+            o = 0;
+        }
+        return o;
+    };
+    std::map<std::string, uint64_t> text_ext; // path string / link target -> its extent
+    auto put_text = [&](const std::string &b) {
+        auto it = text_ext.find(b);
+        if (it != text_ext.end())
+            return it->second;
+        if (b.size() > s.cap)
+            throw HostError("path string larger than the arena");
+        const uint64_t o = place(16, b.size());
+        memcpy(s.a + o, b.data(), b.size());
+        s.ext.push_back(mksnap_extent{o, b.size(), 0, MKSNAP_X_CRC, 0});
+        s.pos = o + b.size();
+        text_ext.emplace(b, n_ext);
+        return n_ext++;
+    };
+    struct Sent { // a file that travelled: extents [first, first + pieces) and their lengths
+        const Seg *seg;
+        uint64_t first;
+        std::vector<uint64_t> piece_len;
+    };
+    std::vector<Sent> sent;
+    std::map<FileKey, size_t> sent_of;
+    auto put_file = [&](const Seg &g) { // CRC is linear: a file may be split across arenas at any 16-byte boundary
+        Sent f{&g, n_ext, {}};
+        for (uint64_t done = 0; done < g.size;) {
+            const uint64_t o = place(512, 4096);
+            const uint64_t n = std::min<uint64_t>(g.size - done, (s.cap - o) / 16 * 16);
+            s.jobs.push_back(ReadJob{g.path, done, n, s.a + o});
+            s.ext.push_back(mksnap_extent{o, n, 0, MKSNAP_X_CRC, 0});
+            ++n_ext;
+            f.piece_len.push_back(n);
+            s.pos = o + n;
+            done += n;
+        }
+        st.bytes_sent += g.size;
+        sent.push_back(std::move(f));
+        return sent.size() - 1;
+    };
+    std::vector<mksnap_crc_use> uses; // grouped by stream, as k_crc_fold prefers them
+    for (size_t k = 0; k < batch.size(); ++k) {
+        const uint32_t slot = (uint32_t)k;
+        const std::vector<Seg> &ss = segs[batch[k]];
+        uint64_t after = 0; // stream bytes after the segment
+        for (const auto &g : ss)
+            after += g.kind == 'F' ? g.size : g.bytes.size();
+        slen[batch[k]] = after;
+        for (const auto &g : ss) {
+            if (g.kind != 'F') {
+                after -= g.bytes.size();
+                if (!g.bytes.empty())
+                    uses.push_back(mksnap_crc_use{after, put_text(g.bytes), slot, 0});
+                continue;
+            }
+            ++st.files_total;
+            st.bytes_total += g.size;
+            after -= g.size;
+            if (g.size == 0)
+                continue;
+            if (cache) { // unchanged since a build that remembered it: no read
+                auto it = cache->files.find(g.path);
+                if (it != cache->files.end() && it->second.dev == g.dev && it->second.ino == g.ino && it->second.size == g.size &&
+                    it->second.mtime_ns == g.mtime_ns && it->second.ctime_ns == g.ctime_ns) {
+                    ++st.files_reused;
+                    uses.push_back(mksnap_crc_use{after, it->second.pure, slot, MKSNAP_U_VALUE});
+                    continue;
+                }
+            }
+            const FileKey key = file_key(g);
+            auto kn = known.find(key); // valued by an earlier session of this plan
+            if (kn != known.end()) {
+                uses.push_back(mksnap_crc_use{after, kn->second, slot, MKSNAP_U_VALUE});
+                continue;
+            }
+            auto so = sent_of.find(key);
+            const Sent &f = sent[so != sent_of.end() ? so->second : (sent_of[key] = put_file(g))];
+            uint64_t a = after + g.size;
+            for (size_t p = 0; p < f.piece_len.size(); ++p) {
+                a -= f.piece_len[p];
+                uses.push_back(mksnap_crc_use{a, f.first + p, slot, 0});
+            }
+        }
+    }
+    s.submit();
+    const auto t_fold = std::chrono::steady_clock::now();
+    for (size_t u0 = 0; u0 < uses.size(); u0 += s.lim.max_extents)
+        ck(eng, mksnap_crc_fold(eng, uses.data() + u0, std::min<uint64_t>(s.lim.max_extents, uses.size() - u0)), "crc fold");
+    mksnap_result res;
+    ck(eng, mksnap_finish(eng, &res), "finish");
+    ms_fold += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_fold).count();
+    std::vector<uint32_t> val(batch.size());
+    uint64_t n_val = 0;
+    ck(eng, mksnap_get_crc_streams(eng, val.data(), val.size(), &n_val), "crc streams");
+    for (size_t k = 0; k < batch.size(); ++k)
+        pure[batch[k]] = k < n_val ? val[k] : 0u; // a stream nothing was folded into is empty
+    if (sent.empty() || !(cache || remember))
+        return;
+    std::vector<uint32_t> ext(n_ext);
+    uint64_t n_got = 0;
+    ck(eng, mksnap_get_extent_crcs(eng, ext.data(), ext.size(), &n_got), "extent crcs");
+    if (n_got != n_ext)
+        throw HostError("internal: extent count mismatch");
+    for (const Sent &f : sent) { // pure(A||B) = pure(A) x^(8|B|) ^ pure(B)
+        uint32_t v = 0;
+        for (size_t p = 0; p < f.piece_len.size(); ++p)
+            v = mksnap_crc_concat(v, ext[f.first + p], f.piece_len[p]);
+        const Seg &g = *f.seg;
+        if (cache)
+            cache->files[g.path] = mkhost_crc_cache::Entry{g.dev, g.ino, g.size, g.mtime_ns, g.ctime_ns, v};
+        if (remember)
+            known[file_key(g)] = v;
+    }
+}
+
+int mkhost_plan_cache_ids(mksnap_t *eng, mkhost_crc_cache *cache, const char *seed, const char *context_dir,
+                          const mkhost_plan_step *steps, size_t n_steps, int n_threads, uint32_t *ids_out,
+                          mkhost_crc_cache_stats *stats, char *err, size_t errlen)
+{
+    try {
+        if (!eng || !seed || !context_dir || (n_steps && (!steps || !ids_out)))
+            throw HostError("null argument");
+        const auto t_start = std::chrono::steady_clock::now();
+        const std::string ctx = go_clean(context_dir);
+        std::vector<std::vector<Seg>> segs(n_steps);
+        std::vector<size_t> walked; // steps that hash context content, in plan order
+        for (size_t i = 0; i < n_steps; ++i) {
+            const mkhost_plan_step &p = steps[i];
+            if (p.kind < MKHOST_STEP_COPY || p.kind > MKHOST_STEP_REMOTE_FROM)
+                throw HostError("step " + std::to_string(i) + ": unknown kind " + std::to_string(p.kind));
+            if (p.kind == MKHOST_STEP_COPY && !(p.from_stage && *p.from_stage)) {
+                if (p.n_paths && !p.from_paths)
+                    throw HostError("step " + std::to_string(i) + ": null from_paths");
+                segs[i] = context_segments(ctx, p.from_paths, p.n_paths, n_threads);
+                walked.push_back(i);
+            }
+        }
+        const double ms_walk = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        std::vector<uint32_t> pure(n_steps, 0);
+        std::vector<uint64_t> slen(n_steps, 0);
+        mkhost_crc_cache_stats st{};
+        std::map<FileKey, uint32_t> known;
+        double ms_fold = 0;
+        const uint64_t slots = engine_limits(eng).max_streams;
+        size_t n_sessions = 0;
+        for (size_t b0 = 0; b0 < walked.size(); b0 += slots, ++n_sessions) {
+            const size_t b1 = (size_t)std::min<uint64_t>(walked.size(), b0 + slots);
+            const std::vector<size_t> batch(walked.begin() + b0, walked.begin() + b1);
+            plan_session(eng, cache, segs, batch, n_threads, known, b1 < walked.size(), pure, slen, st, ms_fold);
+        }
+        // the seed chain, in plan order (createDockerfileSteps: seed = step.CacheID())
+        std::string sd = seed, stage_seed;
+        bool in_remote = false;
+        for (size_t i = 0; i < n_steps; ++i) {
+            const mkhost_plan_step &p = steps[i];
+            const std::string dir = p.directive ? p.directive : "", args = p.args ? p.args : "";
+            const bool remote = p.kind == MKHOST_STEP_REMOTE_FROM;
+            if (remote && !in_remote)
+                stage_seed = sd;
+            else if (!remote && in_remote)
+                sd = stage_seed;
+            in_remote = remote;
+            std::string prefix;
+            if (p.kind == MKHOST_STEP_FROM || remote)
+                prefix = sd + "FROM" + args;
+            else if (p.kind == MKHOST_STEP_BASE)
+                prefix = sd + dir + args + (p.commit ? "true" : "false");
+            else
+                prefix = sd + dir + args;
+            ids_out[i] = mksnap_crc_prepend(prefix.data(), prefix.size(), pure[i], slen[i]);
+            char hex[16];
+            snprintf(hex, sizeof hex, "%x", ids_out[i]);
+            sd = hex;
+        }
+        if (getenv("MKHOST_TRACE"))
+            fprintf(stderr, "[mkhost] plan cacheIDs: %zu steps, %zu walked, %zu sessions; walk %.2f ms, fold + finish %.2f ms, total %.2f ms\n",
+                    n_steps, walked.size(), n_sessions, ms_walk, ms_fold,
+                    std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count());
+        if (stats)
+            *stats = st;
+        return 0;
+    } catch (const std::exception &e) {
+        set_err(err, errlen, std::string("hash context sources: ") + e.what());
+        return -1;
+    }
 }
 
 int mkhost_commit_copy_ops(mksnap_t *eng, const char *root_dir, int64_t now_unix, const mkhost_copy_op *ops, size_t n_ops,
