@@ -170,6 +170,33 @@ int mkhost_memfs_file_digest(mkhost_memfs *m, const char *dst, uint8_t out[32]);
 int mkhost_memfs_commit_copy_ops(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_copy_op *ops, size_t n_ops,
                                  int n_threads, int tar_fd, uint32_t flags, mkhost_layer_result *out, char *err,
                                  size_t errlen);
+/* Incremental layer commit.  Chunks never span files, so a file's chunk digests depend on its bytes (and the CDC
+ * parameters) alone, and the chunk table is the sorted-unique multiset of all of them: the digests of an UNCHANGED file,
+ * remembered from an earlier commit, can join the table (mksnap_chunks_add) instead of the file being chunked again.
+ * "Unchanged" is what it is for the incremental cacheID: same device, inode, size, mtime and ctime (nanoseconds) as when
+ * the file was read.  The result -- entries, tar bytes to tar_fd, TarDigest, root, n_chunks, n_unique -- is that of
+ * mkhost_memfs_commit_copy_ops with the same flags, bit for bit, whenever the remembered digests are current; with
+ * cache == NULL this IS mkhost_memfs_commit_copy_ops.  What is saved depends on the mode: TarDigest is one serial SHA-256
+ * chain over every byte, so by default an unchanged file still travels to the device (the chain reads it) and only the
+ * scan and chunk SHA-256 skip it; under MKHOST_NO_TAR_DIGEST nothing on the device needs it, so its bytes do not cross
+ * PCIe (mksnap_arena_submit_spans), and without tar_fd and MKHOST_MATERIALIZE it is not even read.  Every file chunked
+ * by the commit is remembered.  The cache records the CDC parameters (mksnap_get_cdc); used with an engine cut under
+ * others it starts over, nothing is an error.  One cache per build context, owned by the caller; save/load keep it
+ * between processes.  stats: regular files of the layer and their bytes, files taken from the cache, bytes chunked on
+ * the device, file bytes copied to the device. */
+typedef struct mkhost_chunk_cache mkhost_chunk_cache;
+typedef struct {
+    uint64_t files_total, files_reused;
+    uint64_t bytes_total, bytes_chunked, bytes_uploaded;
+} mkhost_chunk_cache_stats;
+mkhost_chunk_cache *mkhost_chunk_cache_new(void);
+void mkhost_chunk_cache_free(mkhost_chunk_cache *c);
+uint64_t mkhost_chunk_cache_size(const mkhost_chunk_cache *c);
+int mkhost_chunk_cache_save(const mkhost_chunk_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_chunk_cache_load(mkhost_chunk_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_memfs_commit_copy_ops_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chunk_cache *cache, int64_t now_unix,
+                                        const mkhost_copy_op *ops, size_t n_ops, int n_threads, int tar_fd, uint32_t flags,
+                                        mkhost_layer_result *out, mkhost_chunk_cache_stats *stats, char *err, size_t errlen);
 int mkhost_memfs_commit_scan(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int n_threads, int tar_fd, uint32_t flags,
                              mkhost_layer_result *out, char *err, size_t errlen);
 /* Several consecutive layers of ONE build committed in one engine session.  Equivalent to calling

@@ -241,9 +241,39 @@ int mksnap_get_crc_streams(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint6
 /* host arithmetic, no device: checksum.Sum32() of prefix || rest, given pure(rest) and len(rest) */
 uint32_t mksnap_crc_prepend(const void *prefix, uint64_t n, uint32_t pure_rest, uint64_t len_rest);
 
+/* ---- incremental layer commit: chunk digests remembered from an earlier session ----
+ * Chunks never span files (DESIGN.md section 3), so a file's chunk digests depend on its own bytes only, and the table
+ * is the sorted-unique multiset of all of them.  A caller that remembers a file's digests (keyed by file identity, under
+ * the CDC parameters mksnap_get_cdc reports) appends them for an UNCHANGED file with mksnap_chunks_add instead of
+ * submitting the file as a MKSNAP_X_CDC extent; finish sorts, uniques and roots the union, so root, n_chunks and
+ * n_unique equal those of the full pass.  Appended rows join the table in call order behind the chunks of the submits
+ * enqueued before the call (k_chunks_append, stream-ordered); mksnap_get_chunks returns them with end == UINT64_MAX.  At
+ * most MKSNAP_CHUNKS_ADD_MAX rows (32 bytes each) per call: they travel through one pinned staging buffer of that size in
+ * one copy; `digests` may be reused when the call returns.  Rows past max_chunks fail finish with MKSNAP_E_CAPACITY,
+ * like computed chunks.  Call between begin and finish. */
+#define MKSNAP_CHUNKS_ADD_MAX 65536u
+int mksnap_chunks_add(mksnap_t *h, const uint8_t *digests, uint64_t n);
+/* mksnap_arena_submit that copies only the listed spans of arena[0, used) host->device: the bytes the device reads
+ * (MKSNAP_X_CDC / MKSNAP_X_CRC extents, ranges).  A file whose digests are appended and whose bytes are in the arena only
+ * for the host (the layer tar to a file descriptor) then does not cross PCIe.  Spans are ascending, non-overlapping, off
+ * and len multiples of 16, inside [0, used); every extent and range must lie inside one span (MKSNAP_E_INVAL
+ * otherwise).  Device bytes of [0, used) outside the spans are zeroed on the copy stream, so the scan, which still reads
+ * the whole arena, never sees bytes of an earlier submit.  stats.h2d_bytes counts the spans.  mksnap_arena_submit is
+ * the single span [0, used). */
+typedef struct {
+    uint64_t off;
+    uint64_t len;
+} mksnap_span;
+int mksnap_arena_submit_spans(mksnap_t *h, int32_t arena_id, uint64_t used, const mksnap_span *spans, uint64_t n_spans,
+                              const mksnap_extent *extents, uint64_t n_extents, const mksnap_range *ranges,
+                              uint64_t n_ranges);
+/* the handle's effective CDC parameters (defaults filled in): remembered chunk digests are valid only under these */
+int mksnap_get_cdc(const mksnap_t *h, mksnap_cdc_params *out);
+
 /* ---- result tables (valid after mksnap_finish, until the next begin) ---- */
 /* chunk END offsets (exclusive; position in the concatenation of all submitted
- * arenas) and digests, in (submit, extent, position) order. */
+ * arenas) and digests, in (submit, extent, position) order; rows of mksnap_chunks_add
+ * in their place in that order, with end = UINT64_MAX. */
 int mksnap_get_chunks(mksnap_t *h, uint64_t *ends, uint8_t *digests, uint64_t capacity);
 /* sorted-unique 32-byte digest table */
 int mksnap_get_table(mksnap_t *h, uint8_t *table, uint64_t capacity_rows);

@@ -58,6 +58,13 @@ class CrcUse(C.Structure):
 MKSNAP_U_VALUE = 1  # CrcUse.src holds the pure value itself, not an extent index
 
 
+class Span(C.Structure):
+    _fields_ = [("off", C.c_uint64), ("len", C.c_uint64)]
+
+
+MKSNAP_CHUNKS_ADD_MAX = 65536  # rows per mksnap_chunks_add call
+
+
 class Result(C.Structure):
     _fields_ = [("crc_pure", C.c_uint32), ("reserved", C.c_uint32), ("crc_bytes", C.c_uint64),
                 ("cdc_bytes", C.c_uint64), ("n_files", C.c_uint64), ("n_chunks", C.c_uint64),
@@ -100,6 +107,10 @@ SYMBOLS = [
     ("mksnap_crc_fold", C.c_int, [_P, C.POINTER(CrcUse), C.c_uint64]),
     ("mksnap_get_crc_streams", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("mksnap_crc_prepend", C.c_uint32, [C.c_char_p, C.c_uint64, C.c_uint32, C.c_uint64]),
+    ("mksnap_chunks_add", C.c_int, [_P, _P, C.c_uint64]),
+    ("mksnap_arena_submit_spans", C.c_int, [_P, C.c_int32, C.c_uint64, C.POINTER(Span), C.c_uint64, C.POINTER(Extent),
+                                            C.c_uint64, C.POINTER(Range), C.c_uint64]),
+    ("mksnap_get_cdc", C.c_int, [_P, C.POINTER(CdcParams)]),
     ("mksnap_get_chunks", C.c_int, [_P, _P, _P, C.c_uint64]),
     ("mksnap_get_table", C.c_int, [_P, _P, C.c_uint64]),
     ("mksnap_get_stream_digests", C.c_int, [_P, _P, C.c_uint64]),
@@ -248,6 +259,24 @@ class Engine:
     def arena_submit(self, arena_id: int, used: int, extents, ranges=None):
         ea, ne, ra, nr = self._tables(extents, ranges)
         self._ck(self.lib.mksnap_arena_submit(self.h, arena_id, used, ea, ne, ra, nr), "mksnap_arena_submit")
+
+    def arena_submit_spans(self, arena_id: int, used: int, spans, extents, ranges=None):
+        """spans: (off, len) pairs, the only bytes of arena[0, used) that travel; the rest is zeroed on the device."""
+        ea, ne, ra, nr = self._tables(extents, ranges)
+        sa = (Span * max(1, len(spans)))(*[Span(o, n) for o, n in spans])
+        self._ck(self.lib.mksnap_arena_submit_spans(self.h, arena_id, used, sa, len(spans), ea, ne, ra, nr),
+                 "mksnap_arena_submit_spans")
+
+    def chunks_add(self, digests):
+        """Append remembered chunk digests (n x 32 uint8, at most MKSNAP_CHUNKS_ADD_MAX rows) to the session's table."""
+        import numpy as np
+        d = np.ascontiguousarray(digests, dtype=np.uint8).reshape(-1, 32)
+        self._ck(self.lib.mksnap_chunks_add(self.h, d.ctypes.data, d.shape[0]), "mksnap_chunks_add")
+
+    def get_cdc(self) -> CdcParams:
+        p = CdcParams()
+        self._ck(self.lib.mksnap_get_cdc(self.h, C.byref(p)), "mksnap_get_cdc")
+        return p
 
     def device_submit(self, slot: int, used: int, extents, ranges=None):
         ea, ne, ra, nr = self._tables(extents, ranges)

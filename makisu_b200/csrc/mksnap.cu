@@ -129,6 +129,9 @@ struct mksnap {
     CrcUse *d_uses = nullptr;          // mksnap_crc_fold: use table (max_extents rows) and stream values (max_streams),
     uint32_t *d_stream_pure = nullptr; //   allocated by the first fold
     uint64_t fold_streams = 0;         // highest stream slot folded in this session + 1
+    uint8_t *h_add = nullptr;          // mksnap_chunks_add: pinned staging of MKSNAP_CHUNKS_ADD_MAX rows, its device
+    uint8_t *d_add = nullptr;          //   twin and the end of the last copy out of it; allocated by the first call
+    cudaEvent_t ev_add = nullptr;
     bool open_file = false;      // the last submit ended with a MKSNAP_X_MORE extent: the next must start with its continuation
     uint8_t *d_carry = nullptr;  // open chunk of that file (k_carry_out -> k_carry_in)
     uint64_t carry_cap = 0;
@@ -690,6 +693,9 @@ void mksnap_destroy(mksnap_t *h)
     cudaFree(h->d_carry);
     cudaFree(h->d_crc_session);
     cudaFree(h->d_uses); cudaFree(h->d_stream_pure);
+    cudaFreeHost(h->h_add); cudaFree(h->d_add);
+    if (h->ev_add)
+        cudaEventDestroy(h->ev_add);
     cudaFree(h->d_tiles); cudaFree(h->d_part); cudaFree(h->d_pool); cudaFree(h->d_pool_count); cudaFree(h->d_counts); cudaFree(h->d_bases);
     cudaFree(h->d_scan_tmp);
     cudaFree(h->d_order); cudaFree(h->d_chunk_start); cudaFree(h->d_chunk_len); cudaFree(h->d_chunk_end); cudaFree(h->d_digests);
@@ -783,8 +789,19 @@ int mksnap_get_limits(const mksnap_t *h, mksnap_limits *out)
     return 0;
 }
 
+// [off, off + len) inside one of the ascending spans (empty pieces need no bytes)
+static bool in_spans(const mksnap_span *sp, uint64_t n, uint64_t off, uint64_t len)
+{
+    if (len == 0)
+        return true;
+    const mksnap_span *it = std::upper_bound(sp, sp + n, off, [](uint64_t v, const mksnap_span &s) { return v < s.off; });
+    return it != sp && off + len <= (it - 1)->off + (it - 1)->len;
+}
+
+// src != nullptr: the arena comes from that pinned host arena, and of [0, used) only `spans` travel (the rest is zeroed)
 static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_extent *ext, uint64_t n_ext,
-                         const mksnap_range *rng, uint64_t n_rng, HostArena *src)
+                         const mksnap_range *rng, uint64_t n_rng, HostArena *src, const mksnap_span *spans = nullptr,
+                         uint64_t n_spans = 0)
 {
     if (!h->in_session || h->finished)
         return fail(h, MKSNAP_E_STATE, "submit outside begin/finish");
@@ -886,7 +903,17 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         CK(h, cudaStreamWaitEvent(sc, h->ev_slot_free[slot], 0));
     if (src) {
         CK(h, cudaEventRecord(h->ev_copy0, sc));
-        CK(h, cudaMemcpyAsync(d_arena, src->ptr, used, cudaMemcpyHostToDevice, sc));
+        uint64_t at = 0, sent = 0; // bytes before `at` are placed; a gap between spans is zeroed
+        for (uint64_t k = 0; k < n_spans; k++) {
+            if (spans[k].off > at)
+                CK(h, cudaMemsetAsync(d_arena + at, 0, spans[k].off - at, sc));
+            if (spans[k].len)
+                CK(h, cudaMemcpyAsync(d_arena + spans[k].off, src->ptr + spans[k].off, spans[k].len, cudaMemcpyHostToDevice, sc));
+            at = spans[k].off + spans[k].len;
+            sent += spans[k].len;
+        }
+        if (used > at)
+            CK(h, cudaMemsetAsync(d_arena + at, 0, used - at, sc));
         // zero the tail up to the next 512 so row-granular readers see zeros
         const uint64_t padded = std::min<uint64_t>((used + 511) & ~511ull, h->cfg.device_arena_bytes);
         if (padded > used)
@@ -895,7 +922,7 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         CK(h, cudaEventRecord(src->ev_h2d, sc));
         src->in_flight = true;
         src->acquired = false;
-        h->stats.h2d_bytes += used;
+        h->stats.h2d_bytes += sent;
         h->have_h2d_time = true;
     }
     if (n_crc) {
@@ -1026,6 +1053,35 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
     return 0;
 }
 
+int mksnap_arena_submit_spans(mksnap_t *h, int32_t arena_id, uint64_t used, const mksnap_span *spans, uint64_t n_spans,
+                              const mksnap_extent *extents, uint64_t n_extents, const mksnap_range *ranges, uint64_t n_ranges)
+{
+    if (!h)
+        return MKSNAP_E_INVAL;
+    CK(h, cudaSetDevice(h->cfg.device));
+    if (arena_id < 0 || (size_t)arena_id >= h->arenas.size() || !h->arenas[arena_id].acquired)
+        return fail(h, MKSNAP_E_STATE, "arena %d was not acquired", arena_id);
+    if (used > h->cfg.host_arena_bytes)
+        return fail(h, MKSNAP_E_CAPACITY, "used %llu > host arena %llu", (unsigned long long)used,
+                    (unsigned long long)h->cfg.host_arena_bytes);
+    if ((!spans && n_spans) || (!extents && n_extents) || (!ranges && n_ranges))
+        return fail(h, MKSNAP_E_INVAL, "null table");
+    for (uint64_t k = 0, end = 0; k < n_spans; k++) {
+        const mksnap_span &s = spans[k];
+        if ((s.off | s.len) & 15 || s.off < end || s.off > used || s.len > used - s.off)
+            return fail(h, MKSNAP_E_INVAL, "span %llu: not 16-byte aligned, out of order or outside [0, used)", (unsigned long long)k);
+        end = s.off + s.len;
+    }
+    for (uint64_t i = 0; i < n_extents; i++)
+        if (!in_spans(spans, n_spans, extents[i].arena_off, extents[i].len))
+            return fail(h, MKSNAP_E_INVAL, "extent %llu is not inside one of the submitted spans", (unsigned long long)i);
+    for (uint64_t i = 0; i < n_ranges; i++)
+        if (!in_spans(spans, n_spans, ranges[i].arena_off, ranges[i].len))
+            return fail(h, MKSNAP_E_INVAL, "range %llu is not inside one of the submitted spans", (unsigned long long)i);
+    const uint32_t slot = (uint32_t)(h->submit_idx % h->n_slots);
+    return submit_common(h, slot, used, extents, n_extents, ranges, n_ranges, &h->arenas[arena_id], spans, n_spans);
+}
+
 int mksnap_arena_submit(mksnap_t *h, int32_t arena_id, uint64_t used, const mksnap_extent *extents,
                         uint64_t n_extents, const mksnap_range *ranges, uint64_t n_ranges)
 {
@@ -1037,8 +1093,52 @@ int mksnap_arena_submit(mksnap_t *h, int32_t arena_id, uint64_t used, const mksn
     if (used > h->cfg.host_arena_bytes)
         return fail(h, MKSNAP_E_CAPACITY, "used %llu > host arena %llu", (unsigned long long)used,
                     (unsigned long long)h->cfg.host_arena_bytes);
+    const mksnap_span whole{0, used}; // `used` need not be a multiple of 16 here
     const uint32_t slot = (uint32_t)(h->submit_idx % h->n_slots);
-    return submit_common(h, slot, used, extents, n_extents, ranges, n_ranges, &h->arenas[arena_id]);
+    return submit_common(h, slot, used, extents, n_extents, ranges, n_ranges, &h->arenas[arena_id], &whole, 1);
+}
+
+int mksnap_chunks_add(mksnap_t *h, const uint8_t *digests, uint64_t n)
+{
+    if (!h)
+        return MKSNAP_E_INVAL;
+    if (!digests && n)
+        return fail(h, MKSNAP_E_INVAL, "chunks_add: null digest table");
+    if (!h->in_session || h->finished)
+        return fail(h, MKSNAP_E_STATE, "chunks_add outside begin/finish");
+    if (n > MKSNAP_CHUNKS_ADD_MAX)
+        return fail(h, MKSNAP_E_CAPACITY, "chunks_add: %llu rows in one call, at most %u", (unsigned long long)n,
+                    MKSNAP_CHUNKS_ADD_MAX);
+    if (n == 0)
+        return 0;
+    CK(h, cudaSetDevice(h->cfg.device));
+    cudaStream_t s = h->s_comp; // behind the submits enqueued before this call
+    if (!h->h_add) {
+        CK(h, cudaHostAlloc(&h->h_add, (uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32, cudaHostAllocDefault));
+        CK(h, cudaMalloc(&h->d_add, (uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32));
+        CK(h, cudaEventCreateWithFlags(&h->ev_add, cudaEventDisableTiming));
+    } else {
+        CK(h, cudaEventSynchronize(h->ev_add)); // the previous call's copy has left the staging buffer
+    }
+    memcpy(h->h_add, digests, n * 32);
+    CK(h, cudaMemcpyAsync(h->d_add, h->h_add, n * 32, cudaMemcpyHostToDevice, s));
+    CK(h, cudaEventRecord(h->ev_add, s));
+    h->stats.h2d_bytes += n * 32;
+    const uint32_t grid = (uint32_t)std::min<uint64_t>((2 * n + APPEND_THREADS - 1) / APPEND_THREADS, (uint64_t)h->sm_count * 4);
+    k_chunks_append<<<grid, APPEND_THREADS, 0, s>>>(reinterpret_cast<const uint4 *>(h->d_add), (uint32_t)n, h->d_sc,
+                                                    h->max_chunks, reinterpret_cast<uint4 *>(h->d_digests), h->d_chunk_end);
+    LAUNCH_OK(h);
+    k_chunks_commit<<<1, 32, 0, s>>>(h->d_sc, (uint32_t)n, h->max_chunks);
+    LAUNCH_OK(h);
+    return 0;
+}
+
+int mksnap_get_cdc(const mksnap_t *h, mksnap_cdc_params *out)
+{
+    if (!h || !out)
+        return MKSNAP_E_INVAL;
+    *out = h->cfg.cdc; // create() filled in the defaults
+    return 0;
 }
 
 int mksnap_device_arena(mksnap_t *h, uint32_t slot, void **device_ptr, uint64_t *capacity)

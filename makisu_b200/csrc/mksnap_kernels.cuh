@@ -5,6 +5,7 @@
 //   K1  k_roll_scan       Roll-32 candidate scan [+ row CRCs]    (HBM-read bound)
 //   K1b k_select_cuts     min/normal/max cut selection per file  (latency, tiny)
 //   K2  k_sha256_ranges   SHA-256 of the chunks                  (int-ALU bound)
+//   K2a k_chunks_append   remembered chunk digests into the table (copy, tiny)
 //       (the serial layer-tar streams and the Merkle levels of the table root
 //        are K4, mksnap_sha_stream.cuh)
 //   K3  radix sort / unique of 256-bit digests                   (HBM, tiny)
@@ -1139,6 +1140,44 @@ __global__ void k_batch_end(SessionCounters *sc)
             sc->n_chunks += sc->batch_chunks;
         sc->batch_chunks = 0;
         sc->work = 0;
+    }
+}
+
+// K2a: chunk digests remembered from an earlier session (mksnap_chunks_add) join the chunk table behind the chunks of
+// the submits enqueued before them.  Chunks never span files, so a file's digests depend on its bytes alone and the
+// sorted-unique table -- hence the root -- of the union is that of a full pass.  k_chunks_append writes rows
+// [n_chunks, n_chunks + n) (digest, end = UINT64_MAX so that callers of mksnap_get_chunks can tell them from computed
+// chunks); k_chunks_commit then publishes them.  Both apply the same test first: a session that already failed, or rows
+// that would run past max_chunks, write nothing, and k_chunks_commit sets the table-overflow bit (finish reports
+// MKSNAP_E_CAPACITY).  Two launches instead of one keep the counter read of every CTA ahead of the update.
+constexpr int APPEND_THREADS = 256;
+
+__device__ __forceinline__ bool chunks_append_refused(const SessionCounters *sc, uint32_t n, uint64_t max_chunks)
+{
+    return sc->err != 0 || sc->n_chunks + n > max_chunks;
+}
+
+__global__ void __launch_bounds__(APPEND_THREADS)
+k_chunks_append(const uint4 *__restrict__ rows, uint32_t n, const SessionCounters *__restrict__ sc, uint64_t max_chunks,
+                uint4 *__restrict__ digests, uint64_t *__restrict__ chunk_end)
+{
+    if (chunks_append_refused(sc, n, max_chunks))
+        return;
+    const uint64_t base = sc->n_chunks;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < 2 * n; i += gridDim.x * blockDim.x) { // 2 x 16 B per row
+        digests[2 * base + i] = rows[i];
+        if (!(i & 1u))
+            chunk_end[base + i / 2] = ~0ull;
+    }
+}
+
+__global__ void k_chunks_commit(SessionCounters *sc, uint32_t n, uint64_t max_chunks)
+{
+    if (threadIdx.x == 0 && blockIdx.x == 0) {
+        if (!chunks_append_refused(sc, n, max_chunks))
+            sc->n_chunks += n;
+        else if (!sc->err)
+            sc->err |= 2u;
     }
 }
 

@@ -30,6 +30,11 @@ class CrcCacheStats(C.Structure):
     _fields_ = [("files_total", C.c_uint64), ("files_reused", C.c_uint64), ("bytes_total", C.c_uint64), ("bytes_sent", C.c_uint64)]
 
 
+class ChunkCacheStats(C.Structure):
+    _fields_ = [("files_total", C.c_uint64), ("files_reused", C.c_uint64), ("bytes_total", C.c_uint64),
+                ("bytes_chunked", C.c_uint64), ("bytes_uploaded", C.c_uint64)]
+
+
 class LayerSpec(C.Structure):
     _fields_ = [("ops", C.POINTER(CopyOp)), ("n_ops", C.c_size_t), ("tar_fd", C.c_int)]
 
@@ -70,6 +75,14 @@ SYMBOLS = [
     ("mkhost_memfs_file_digest", C.c_int, [_P, C.c_char_p, C.POINTER(C.c_uint8)]),
     ("mkhost_memfs_commit_copy_ops", C.c_int, [_P, _P, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_int, C.c_int, C.c_uint32,
                                                C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
+    ("mkhost_chunk_cache_new", _P, []),
+    ("mkhost_chunk_cache_free", None, [_P]),
+    ("mkhost_chunk_cache_size", C.c_uint64, [_P]),
+    ("mkhost_chunk_cache_save", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_chunk_cache_load", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_memfs_commit_copy_ops_cached", C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_int, C.c_int,
+                                                      C.c_uint32, C.POINTER(LayerResult), C.POINTER(ChunkCacheStats),
+                                                      C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_commit_layers", C.c_int, [_P, _P, C.c_int64, C.POINTER(LayerSpec), C.c_size_t, C.c_int, C.c_uint32,
                                              C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_commit_scan", C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, C.c_uint32, C.POINTER(LayerResult),
@@ -318,6 +331,18 @@ class MemFS:
             raise HostError(err.value.decode())
         return _layer_dict(out)
 
+    def commit_copy_ops_cached(self, eng: abi.Engine, cache: Optional["ChunkCache"], now_unix: int,
+                               ops: Sequence[CopyOperation], n_threads: int = 0, tar_fd: int = -1, flags: int = 0):
+        """commit_copy_ops with remembered chunk digests for unchanged files -> (layer dict, stats dict).  The layer is
+        the one commit_copy_ops returns; cache None = no cache."""
+        err, out, st = C.create_string_buffer(1024), LayerResult(), ChunkCacheStats()
+        arr, keep = _ops(ops)
+        if load().mkhost_memfs_commit_copy_ops_cached(self.h, eng.h, cache.h if cache is not None else None, now_unix, arr,
+                                                      len(ops), n_threads, tar_fd, flags, C.byref(out), C.byref(st), err,
+                                                      len(err)):
+            raise HostError(err.value.decode())
+        return _layer_dict(out), {k: getattr(st, k) for k, _ in ChunkCacheStats._fields_}
+
     def commit_layers(self, eng: abi.Engine, now_unix: int, layers: Sequence[Sequence[CopyOperation]], n_threads: int = 0,
                       tar_fds: Optional[Sequence[int]] = None, flags: int = 0):
         """Consecutive layers of one build in ONE engine session (all TarDigest chains advance together)."""
@@ -446,3 +471,33 @@ class CrcCache:
         if rc:
             raise HostError(err.value.decode())
         return crc.value, slen.value, {k: getattr(st, k) for k, _ in CrcCacheStats._fields_}
+
+
+class ChunkCache:
+    """Chunk digests per source file, remembered between builds: a layer commit takes an unchanged file's digests from
+    here instead of chunking it again (include/mkhost.h, "Incremental layer commit"; MemFS.commit_copy_ops_cached)."""
+
+    def __init__(self, path: Optional[str] = None):
+        self.h = load().mkhost_chunk_cache_new()
+        if path is not None and os.path.exists(path):
+            self.load(path)
+
+    def __len__(self):
+        return int(load().mkhost_chunk_cache_size(self.h))
+
+    def load(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_chunk_cache_load(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def save(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_chunk_cache_save(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            load().mkhost_chunk_cache_free(self.h)
+            self.h = None
+
+    __del__ = close

@@ -59,11 +59,15 @@ std::string errno_str(const std::string &what, const std::string &path)
 // pure(file content) per context file, remembered between builds (incremental cacheID, include/mkhost.h)
 struct mkhost_crc_cache {
     struct Entry {
-        uint64_t dev, ino, size;
-        int64_t mtime_ns, ctime_ns;
+        FileId id;
         uint32_t pure;
     };
     std::map<std::string, Entry> files; // key: absolute path
+};
+
+// chunk digests per source file, remembered between builds (incremental layer commit, include/mkhost.h)
+struct mkhost_chunk_cache {
+    ChunkMemo memo;
 };
 
 // persistent snapshot.MemFS mirror (layers accumulate in the merged tree, like context.BuildContext.MemFS)
@@ -210,10 +214,19 @@ int mkhost_memfs_commit_copy_ops(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
                                  int n_threads, int tar_fd, uint32_t flags, mkhost_layer_result *out, char *err,
                                  size_t errlen)
 {
+    return mkhost_memfs_commit_copy_ops_cached(m, eng, nullptr, now_unix, ops, n_ops, n_threads, tar_fd, flags, out, nullptr,
+                                               err, errlen);
+}
+
+int mkhost_memfs_commit_copy_ops_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chunk_cache *cache, int64_t now_unix,
+                                        const mkhost_copy_op *ops, size_t n_ops, int n_threads, int tar_fd, uint32_t flags,
+                                        mkhost_layer_result *out, mkhost_chunk_cache_stats *stats, char *err, size_t errlen)
+{
     try {
         m->fs.set_now(now_unix);
+        ChunkMemo *memo = cache ? &cache->memo : nullptr;
         if (!(flags & MKHOST_MATERIALIZE)) {
-            commit_layer(eng, m->fs.add_layer_by_copy_ops(ops, n_ops), n_threads, tar_fd, flags, out, &m->fs);
+            commit_layer(eng, m->fs.add_layer_by_copy_ops(ops, n_ops), n_threads, tar_fd, flags, out, &m->fs, nullptr, memo, stats);
             return 0;
         }
         // SURVEY section 8f-4: the copy onto the file system (CopyOperation.Execute) and the layer share one read of the
@@ -247,7 +260,8 @@ int mkhost_memfs_commit_copy_ops(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
                 deferred.erase(range.first, range.second);
             }
         };
-        commit_layer(eng, m->fs.add_layer_by_copy_ops(ops, n_ops), n_threads, tar_fd, flags, out, &m->fs, write_from_arena);
+        commit_layer(eng, m->fs.add_layer_by_copy_ops(ops, n_ops), n_threads, tar_fd, flags, out, &m->fs, write_from_arena, memo,
+                     stats);
         for (const auto &kv : deferred)
             copiers[kv.second.copier].finish_regular(kv.second.st, kv.first, kv.second.dst, nullptr, 0);
         return 0;
@@ -515,8 +529,7 @@ static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc
             st.bytes_total += g.size;
             if (cache) { // unchanged since a build that remembered it: fold pure(content) in, send nothing
                 auto it = cache->files.find(g.path);
-                if (it != cache->files.end() && it->second.dev == g.dev && it->second.ino == g.ino && it->second.size == g.size &&
-                    it->second.mtime_ns == g.mtime_ns && it->second.ctime_ns == g.ctime_ns) {
+                if (it != cache->files.end() && it->second.id == g.id) {
                     after -= g.size;
                     ck(eng, mksnap_crc_add(eng, it->second.pure, g.size, after), "crc add");
                     ++st.files_reused;
@@ -568,8 +581,7 @@ static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc
                 uint32_t v = 0; // pure of the empty string
                 for (size_t k = 0; k < f.piece_len.size(); ++k)
                     v = mksnap_crc_concat(v, pure[f.first + k], f.piece_len[k]);
-                cache->files[f.seg->path] =
-                    mkhost_crc_cache::Entry{f.seg->dev, f.seg->ino, f.seg->size, f.seg->mtime_ns, f.seg->ctime_ns, v};
+                cache->files[f.seg->path] = mkhost_crc_cache::Entry{f.seg->id, v};
             }
         }
         if (stats)
@@ -603,9 +615,7 @@ int mkhost_crc_cache_save(const mkhost_crc_cache *c, const char *path, char *err
     fprintf(f, "mkhost-crc-cache 1\n");
     for (const auto &kv : c->files) // path last: it may hold spaces (newlines in file names are not cached)
         if (kv.first.find('\n') == std::string::npos)
-            fprintf(f, "%llu %llu %llu %lld %lld %08x %s\n", (unsigned long long)kv.second.dev, (unsigned long long)kv.second.ino,
-                    (unsigned long long)kv.second.size, (long long)kv.second.mtime_ns, (long long)kv.second.ctime_ns, kv.second.pure,
-                    kv.first.c_str());
+            fprintf(f, "%s %08x %s\n", file_id_text(kv.second.id).c_str(), kv.second.pure, kv.first.c_str());
     const bool ok = fclose(f) == 0;
     if (!ok)
         set_err(err, errlen, std::string("save crc cache: ") + strerror(errno));
@@ -626,21 +636,92 @@ int mkhost_crc_cache_load(mkhost_crc_cache *c, const char *path, char *err, size
     while (ok && (n = getline(&line, &cap, f)) > 0) {
         if (line[n - 1] == '\n')
             line[--n] = 0;
-        unsigned long long dev, ino, size;
-        long long mt, ct;
+        FileId id;
         unsigned pure;
-        int used = 0;
-        if (sscanf(line, "%llu %llu %llu %lld %lld %x %n", &dev, &ino, &size, &mt, &ct, &pure, &used) != 6 || used <= 0 || used >= n) {
+        int used = 0, used2 = 0;
+        if (!parse_file_id(line, &id, &used) || sscanf(line + used, " %x %n", &pure, &used2) != 1 || used2 <= 0 ||
+            used + used2 >= n) {
             ok = false;
             break;
         }
-        c->files[line + used] = mkhost_crc_cache::Entry{dev, ino, size, mt, ct, (uint32_t)pure};
+        c->files[line + used + used2] = mkhost_crc_cache::Entry{id, (uint32_t)pure};
     }
     free(line);
     fclose(f);
     if (!ok)
         set_err(err, errlen, "load crc cache: not a mkhost-crc-cache file");
     return ok ? 0 : -1;
+}
+
+mkhost_chunk_cache *mkhost_chunk_cache_new(void) { return new mkhost_chunk_cache; }
+void mkhost_chunk_cache_free(mkhost_chunk_cache *c) { delete c; }
+uint64_t mkhost_chunk_cache_size(const mkhost_chunk_cache *c) { return c ? c->memo.files.size() : 0; }
+
+// "mkhost-chunk-cache 1 <min> <normal> <max> <strict bits> <loose bits>", then per file a line
+// "<dev> <ino> <size> <mtime ns> <ctime ns> <chunks> <path>" followed by its digests, 32 raw bytes per chunk
+int mkhost_chunk_cache_save(const mkhost_chunk_cache *c, const char *path, char *err, size_t errlen)
+{
+    FILE *f = c && path ? fopen(path, "wb") : nullptr;
+    if (!f) {
+        set_err(err, errlen, std::string("save chunk cache: ") + strerror(errno));
+        return -1;
+    }
+    const mksnap_cdc_params &p = c->memo.cdc;
+    fprintf(f, "mkhost-chunk-cache 1 %u %u %u %u %u\n", p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits);
+    for (const auto &kv : c->memo.files) { // newlines in file names are not cached
+        if (kv.first.find('\n') != std::string::npos)
+            continue;
+        fprintf(f, "%s %zu %s\n", file_id_text(kv.second.id).c_str(), kv.second.digests.size() / 32, kv.first.c_str());
+        fwrite(kv.second.digests.data(), 1, kv.second.digests.size(), f);
+    }
+    const bool ok = !ferror(f) && fclose(f) == 0;
+    if (!ok)
+        set_err(err, errlen, std::string("save chunk cache: ") + strerror(errno));
+    return ok ? 0 : -1;
+}
+
+int mkhost_chunk_cache_load(mkhost_chunk_cache *c, const char *path, char *err, size_t errlen)
+{
+    FILE *f = c && path ? fopen(path, "rb") : nullptr;
+    if (!f) {
+        set_err(err, errlen, std::string("load chunk cache: ") + strerror(errno));
+        return -1;
+    }
+    char *line = nullptr;
+    size_t cap = 0;
+    mksnap_cdc_params p{};
+    ssize_t n = getline(&line, &cap, f);
+    bool ok = n > 0 && sscanf(line, "mkhost-chunk-cache 1 %u %u %u %u %u", &p.min_size, &p.normal_size, &p.max_size,
+                              &p.strict_bits, &p.loose_bits) == 5;
+    std::map<std::string, ChunkMemo::Entry> files;
+    while (ok && (n = getline(&line, &cap, f)) > 0) {
+        if (line[n - 1] == '\n')
+            line[--n] = 0;
+        ChunkMemo::Entry e;
+        unsigned long long rows = 0;
+        int used = 0, used2 = 0;
+        if (!parse_file_id(line, &e.id, &used) || sscanf(line + used, " %llu %n", &rows, &used2) != 1 || used2 <= 0 ||
+            used + used2 >= n || rows > (uint64_t)e.id.size) { // a chunk holds at least one byte
+            ok = false;
+            break;
+        }
+        e.digests.resize(32 * rows);
+        ok = fread(e.digests.data(), 1, e.digests.size(), f) == e.digests.size();
+        files[line + used + used2] = std::move(e);
+    }
+    free(line);
+    fclose(f);
+    if (!ok) {
+        set_err(err, errlen, "load chunk cache: not a mkhost-chunk-cache file");
+        return -1;
+    }
+    if (memcmp(&p, &c->memo.cdc, sizeof p) != 0) { // entries cut under other parameters do not mix with these
+        c->memo.files.clear();
+        c->memo.cdc = p; // a commit under other parameters starts over (ChunkMemo::bind)
+    }
+    for (auto &kv : files)
+        c->memo.files[kv.first] = std::move(kv.second);
+    return 0;
 }
 
 int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const void *prefix, size_t prefix_len,
@@ -659,7 +740,7 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
 // Every distinct path string / link target and every file not yet valued travels once as CRC extents (crc_suffix 0:
 // only pure(extent) is wanted); each occurrence in a stream becomes a use of those extents, or of a known value.
 using FileKey = std::tuple<std::string, uint64_t, uint64_t, uint64_t, int64_t, int64_t>; // path, dev, ino, size, mtime, ctime
-static FileKey file_key(const Seg &g) { return FileKey{g.path, g.dev, g.ino, g.size, g.mtime_ns, g.ctime_ns}; }
+static FileKey file_key(const Seg &g) { return FileKey{g.path, g.id.dev, g.id.ino, g.size, g.id.mtime_ns, g.id.ctime_ns}; }
 
 static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vector<std::vector<Seg>> &segs,
                          const std::vector<size_t> &batch, int n_threads, std::map<FileKey, uint32_t> &known,
@@ -738,8 +819,7 @@ static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vect
                 continue;
             if (cache) { // unchanged since a build that remembered it: no read
                 auto it = cache->files.find(g.path);
-                if (it != cache->files.end() && it->second.dev == g.dev && it->second.ino == g.ino && it->second.size == g.size &&
-                    it->second.mtime_ns == g.mtime_ns && it->second.ctime_ns == g.ctime_ns) {
+                if (it != cache->files.end() && it->second.id == g.id) {
                     ++st.files_reused;
                     uses.push_back(mksnap_crc_use{after, it->second.pure, slot, MKSNAP_U_VALUE});
                     continue;
@@ -785,7 +865,7 @@ static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vect
             v = mksnap_crc_concat(v, ext[f.first + p], f.piece_len[p]);
         const Seg &g = *f.seg;
         if (cache)
-            cache->files[g.path] = mkhost_crc_cache::Entry{g.dev, g.ino, g.size, g.mtime_ns, g.ctime_ns, v};
+            cache->files[g.path] = mkhost_crc_cache::Entry{g.id, v};
         if (remember)
             known[file_key(g)] = v;
     }
