@@ -222,12 +222,12 @@ size_t mkhost_memfs_describe_copy_ops(mkhost_memfs *m, int64_t now_unix, const m
 size_t mkhost_memfs_describe_scan(mkhost_memfs *m, int64_t now_unix, char *out, size_t cap, char *err, size_t errlen);
 
 /* UpdateFromTarReader(r, untar=false) (lib/snapshot/mem_fs.go:165-255; FROM / cache-hit path, from_step.go:118-134):
- * merge an UNCOMPRESSED layer tar read from tar_fd (file or pipe; gunzip stays in Go, lib/tario/gzip.go) into the tree,
+ * merge a layer tar read from tar_fd (file or pipe; uncompressed, or gzip with MKHOST_GUNZIP below) into the tree,
  * hard links in a second pass, nothing written to disk.  The stream goes through the pinned arenas once:
  * out->tar_digest = SHA-256 of every byte read up to EOF (the layer's DiffID: compare with the image config to
  * verify the pulled blob, lib/docker/image/digest.go:42-50), out->root / n_chunks / n_unique = chunk table of the
  * regular-file members (so base layers join the chunk-granular dedup), out->n_entries = headers merged (the
- * count the reference logs).  flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS, MKHOST_UNTAR.  A regular-file member
+ * count the reference logs).  flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS, MKHOST_UNTAR, MKHOST_GUNZIP.  A regular-file member
  * larger than one arena travels in pieces (MKSNAP_X_MORE / MKSNAP_X_CONT); only MKHOST_UNTAR, which writes a member
  * from one contiguous body, still needs every member to fit an arena. */
 int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
@@ -241,6 +241,12 @@ size_t mkhost_memfs_describe_update_from_tar(mkhost_memfs *m, int64_t now_unix, 
  * last; tario.ApplyHeader sets owner, mode and mtime; parent directory mtimes are restored).  On the GPU path the file
  * bodies are written straight from the arena that is being digested. */
 #define MKHOST_UNTAR 32u
+/* MKHOST_GUNZIP (flag of mkhost_memfs_update_from_tar): tar_fd carries the blob as the image store holds it, gzip
+ * (tario.NewGzipReader + UpdateFromTarReader, from_step.go:118-134, build_node.go:131-148).  The blob is read whole and
+ * decompressed on the device (mksnap_gunzip_open / _read, one window at a time); everything downstream is that of the
+ * uncompressed stream: the DiffID is the SHA-256 of the decompressed tar.  Combines with every other flag.  Malformed
+ * gzip data fails the call.  The describe functions read uncompressed tars only. */
+#define MKHOST_GUNZIP 64u
 size_t mkhost_memfs_describe_update_from_tar_ex(mkhost_memfs *m, int64_t now_unix, int tar_fd, uint32_t flags, char *out,
                                                 size_t cap, char *err, size_t errlen);
 

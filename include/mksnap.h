@@ -45,7 +45,8 @@ enum {
     MKSNAP_E_NOMEM = -3,    /* allocation failed */
     MKSNAP_E_CAPACITY = -4, /* batch / table exceeds a configured capacity */
     MKSNAP_E_STATE = -5,    /* call out of sequence */
-    MKSNAP_E_NCCL = -6      /* NCCL unavailable or failed */
+    MKSNAP_E_NCCL = -6,     /* NCCL unavailable or failed */
+    MKSNAP_E_DATA = -7      /* malformed compressed data */
 };
 
 typedef struct mksnap mksnap_t;
@@ -269,6 +270,44 @@ int mksnap_arena_submit_spans(mksnap_t *h, int32_t arena_id, uint64_t used, cons
                               uint64_t n_ranges);
 /* the handle's effective CDC parameters (defaults filled in): remembered chunk digests are valid only under these */
 int mksnap_get_cdc(const mksnap_t *h, mksnap_cdc_params *out);
+
+/* ---- gunzip: decompress a gzip blob on the device (replaces tario.NewGzipReader in FromStep.Execute,
+ * lib/builder/step/from_step.go:118-134, and buildNode.applyLayer, lib/builder/build_node.go:131-148) ----
+ * mksnap_gunzip_open copies the whole blob to the device, finds every candidate segment start (the byte after each
+ * `00 00 FF FF`, the empty stored block of a sync / full flush, and each member body start), decodes from all of them
+ * in parallel without output, links the true chain of segments member by member (trailers, next header) and fills
+ * *info.  mksnap_gunzip_read then hands out the decompressed stream in order: `got` < `cap` only at the end (0 once
+ * everything was read).  The output is produced one window of whole segments at a time: decode to 16-bit symbols,
+ * resolve back-references across segments, CRC-32 each member piece with the K0 kernel, copy to `dst`.
+ * Independent of begin / finish: a gunzip may be open while an ingest session on the same handle is, so the host can
+ * feed the decompressed stream into arenas; calls are serialised by the caller as everywhere else.  One gunzip per
+ * handle at a time (open on an open one: MKSNAP_E_STATE).
+ * Device memory is allocated at open and freed at close / destroy: the blob and its candidate tables (<= 11 * gz_len),
+ * plus one output window of max(256 MiB, largest segment) at 3 bytes per output byte, and a pinned host copy of the
+ * window (reads are host copies; one D2H per window).  A blob without flush points is one segment per member, so there
+ * the window is as large as the largest member.  Blobs of 16 GiB or more are refused (MKSNAP_E_CAPACITY).  Only the
+ * first member body is a scanned start: each later member's first segment is decoded when the link reaches it, one
+ * device launch per member.  The gunzip runs on a stream of its own, so window decodes do not wait behind the work of
+ * an open session.
+ * Acceptance is that of Go's compress/gzip in multistream mode: zlib's inflate for the DEFLATE data; FNAME / FCOMMENT
+ * at most 511 bytes; FHCRC checked; whatever follows a member must be another member header (trailing garbage and zero
+ * padding are errors).  Malformed headers or DEFLATE data fail open with MKSNAP_E_DATA; a distance before the start of
+ * its member, or a CRC-32 / ISIZE mismatch, fails the read that reaches the end of that member (bytes before it are
+ * delivered).  After any error the handle stays usable: close, then open again. */
+typedef struct {
+    uint64_t gz_bytes, out_bytes;   /* blob length, decompressed length over all members */
+    uint64_t n_members, n_segments; /* gzip members; independently decoded pieces (>= n_members) */
+} mksnap_gunzip_info;
+int mksnap_gunzip_open(mksnap_t *h, const void *gz, uint64_t gz_len, mksnap_gunzip_info *info);
+int mksnap_gunzip_read(mksnap_t *h, void *dst, uint64_t cap, uint64_t *got); /* next bytes of the decompressed stream; 0 at the end */
+int mksnap_gunzip_close(mksnap_t *h);
+/* device time of the open gunzip so far (CUDA events on the compute stream): candidate scan, count decodes (including
+ * the re-decodes of starts on the chain, counted in extra_decodes), write decodes, resolve + narrow, member CRC-32 */
+typedef struct {
+    float ms_scan, ms_count, ms_write, ms_resolve, ms_crc;
+    uint32_t extra_decodes;
+} mksnap_gunzip_times;
+int mksnap_gunzip_get_times(mksnap_t *h, mksnap_gunzip_times *out);
 
 /* ---- result tables (valid after mksnap_finish, until the next begin) ---- */
 /* chunk END offsets (exclusive; position in the concatenation of all submitted

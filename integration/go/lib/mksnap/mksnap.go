@@ -21,8 +21,10 @@ package mksnap
 import "C"
 
 import (
+	"bytes"
 	"encoding/hex"
 	"fmt"
+	"io"
 	"os"
 	"runtime"
 	"unsafe"
@@ -182,6 +184,7 @@ const (
 	FileDigests uint32 = 2
 	ScanContent uint32 = 4
 	Materialize uint32 = 8
+	Gunzip      uint32 = 64 // UpdateFromTar: tarIn is the gzip blob as the image store holds it, decompressed on the GPU
 )
 
 // CommitCopyOps = MemFS.AddLayerByCopyOps + commitLayer's tar/SHA-256 half (mem_fs.go:276-289, common.go:35-63).
@@ -249,8 +252,22 @@ func (fs *MemFS) CommitLayers(e *Engine, now int64, layers [][]CopyOp, tarOuts [
 	return res, nil
 }
 
-// UpdateFromTar = MemFS.UpdateFromTarReader (mem_fs.go:165-255) on an UNCOMPRESSED tar stream (gunzip stays Go):
-// the blob's DiffID and the chunk table come back; untar also writes the members under the root from the arena.
+// HasFlushPoints reports whether the gzip blob in f carries a flush marker (00 00 FF FF, the empty stored block pgzip
+// ends every 1 MiB block with) in its first 2 MiB: the blobs makisu writes itself (tario.NewGzipWriter) do once they
+// hold more than one block; gzip-CLI and most registry layers never do.  Only such blobs decode in parallel on the
+// device (UpdateFromTar with Gunzip); any other blob is one GPU thread's work.  f is left at offset 0.
+func HasFlushPoints(f *os.File) (bool, error) {
+	buf := make([]byte, 2<<20)
+	n, err := f.ReadAt(buf, 0)
+	if err != nil && err != io.EOF {
+		return false, err
+	}
+	return bytes.Contains(buf[:n], []byte{0, 0, 0xFF, 0xFF}), nil
+}
+
+// UpdateFromTar = MemFS.UpdateFromTarReader (mem_fs.go:165-255) on a tar stream, uncompressed or, with Gunzip, the
+// gzip blob itself (no tario.NewGzipReader): the DiffID of the tar and the chunk table come back; untar also writes the
+// members under the root from the arena.
 func (fs *MemFS) UpdateFromTar(e *Engine, now int64, tarIn *os.File, untar bool, flags uint32) (LayerResult, error) {
 	if untar {
 		flags |= 32 // MKHOST_UNTAR

@@ -19,7 +19,9 @@ MKSNAP_X_CDC = 2
 MKSNAP_X_MORE = 4   # CDC extent whose file continues in the next submit (reserved = bytes that follow)
 MKSNAP_X_CONT = 8   # CDC extent that continues the MORE extent of the previous submit
 
-ERRORS = {0: "OK", -1: "E_INVAL", -2: "E_CUDA", -3: "E_NOMEM", -4: "E_CAPACITY", -5: "E_STATE", -6: "E_NCCL"}
+ERRORS = {0: "OK", -1: "E_INVAL", -2: "E_CUDA", -3: "E_NOMEM", -4: "E_CAPACITY", -5: "E_STATE", -6: "E_NCCL",
+          -7: "E_DATA"}
+MKSNAP_E_DATA = -7  # malformed compressed data (mksnap_gunzip_*)
 
 
 class MksnapError(RuntimeError):
@@ -84,6 +86,16 @@ class Limits(C.Structure):
                 ("n_device_slots", C.c_uint32), ("carry_bytes", C.c_uint64)]
 
 
+class GunzipInfo(C.Structure):
+    _fields_ = [("gz_bytes", C.c_uint64), ("out_bytes", C.c_uint64), ("n_members", C.c_uint64),
+                ("n_segments", C.c_uint64)]
+
+
+class GunzipTimes(C.Structure):
+    _fields_ = [("ms_scan", C.c_float), ("ms_count", C.c_float), ("ms_write", C.c_float), ("ms_resolve", C.c_float),
+                ("ms_crc", C.c_float), ("extra_decodes", C.c_uint32)]
+
+
 # every symbol include/mksnap.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -111,6 +123,10 @@ SYMBOLS = [
     ("mksnap_arena_submit_spans", C.c_int, [_P, C.c_int32, C.c_uint64, C.POINTER(Span), C.c_uint64, C.POINTER(Extent),
                                             C.c_uint64, C.POINTER(Range), C.c_uint64]),
     ("mksnap_get_cdc", C.c_int, [_P, C.POINTER(CdcParams)]),
+    ("mksnap_gunzip_open", C.c_int, [_P, _P, C.c_uint64, C.POINTER(GunzipInfo)]),
+    ("mksnap_gunzip_read", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("mksnap_gunzip_close", C.c_int, [_P]),
+    ("mksnap_gunzip_get_times", C.c_int, [_P, C.POINTER(GunzipTimes)]),
     ("mksnap_get_chunks", C.c_int, [_P, _P, _P, C.c_uint64]),
     ("mksnap_get_table", C.c_int, [_P, _P, C.c_uint64]),
     ("mksnap_get_stream_digests", C.c_int, [_P, _P, C.c_uint64]),
@@ -277,6 +293,30 @@ class Engine:
         p = CdcParams()
         self._ck(self.lib.mksnap_get_cdc(self.h, C.byref(p)), "mksnap_get_cdc")
         return p
+
+    def gunzip_open(self, blob) -> GunzipInfo:
+        """Start decompressing a gzip blob (bytes-like) on the device; the blob may be dropped when this returns."""
+        b = memoryview(blob).cast("B")
+        buf = (C.c_uint8 * max(1, len(b))).from_buffer_copy(b) if len(b) else (C.c_uint8 * 1)()
+        info = GunzipInfo()
+        self._ck(self.lib.mksnap_gunzip_open(self.h, buf, len(b), C.byref(info)), "mksnap_gunzip_open")
+        return info
+
+    def gunzip_read(self, into) -> int:
+        """Fill the writable buffer `into` with the next decompressed bytes; returns how many (short only at the end)."""
+        m = memoryview(into).cast("B")
+        got = C.c_uint64()
+        ptr = (C.c_uint8 * len(m)).from_buffer(m) if len(m) else None
+        self._ck(self.lib.mksnap_gunzip_read(self.h, ptr, len(m), C.byref(got)), "mksnap_gunzip_read")
+        return got.value
+
+    def gunzip_close(self):
+        self._ck(self.lib.mksnap_gunzip_close(self.h), "mksnap_gunzip_close")
+
+    def gunzip_times(self) -> GunzipTimes:
+        t = GunzipTimes()
+        self._ck(self.lib.mksnap_gunzip_get_times(self.h, C.byref(t)), "mksnap_gunzip_get_times")
+        return t
 
     def device_submit(self, slot: int, used: int, extents, ranges=None):
         ea, ne, ra, nr = self._tables(extents, ranges)

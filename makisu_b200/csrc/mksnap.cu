@@ -73,6 +73,8 @@ struct NcclApi {
 
 } // namespace
 
+struct mksnap_gunzip_state; // mksnap_inflate.cuh
+
 struct mksnap {
     mksnap_config cfg;
     CdcParamsDev prm;
@@ -171,9 +173,13 @@ struct mksnap {
     cudaEvent_t ev_fin[4];
     bool have_submit_times = false, have_h2d_time = false, have_fin_times = false, have_gather_time = false;
     mksnap_stats_t stats;
+
+    mksnap_gunzip_state *gz = nullptr; // open gunzip (mksnap_gunzip_open .. close), independent of the session
 };
 
 namespace {
+
+void gz_free(mksnap *h); // mksnap_inflate.cuh
 
 int fail(mksnap *h, int code, const char *fmt, ...)
 {
@@ -668,6 +674,7 @@ void mksnap_destroy(mksnap_t *h)
         return;
     cudaSetDevice(h->cfg.device);
     cudaDeviceSynchronize();
+    gz_free(h);
     if (h->comm && h->nccl.CommDestroy)
         h->nccl.CommDestroy(h->comm);
     for (uint32_t s = 0; s < MAX_SLOTS; s++) {
@@ -1463,3 +1470,5 @@ int mksnap_stats(mksnap_t *h, mksnap_stats_t *out)
 #include "mksnap_comm.inc"
 
 } // extern "C"
+
+#include "mksnap_inflate.cuh"

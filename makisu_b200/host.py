@@ -266,6 +266,7 @@ MKHOST_SCAN_CONTENT = 4   # content-aware AddLayerByScan (implies FILE_DIGESTS)
 MKHOST_MATERIALIZE = 8    # commit_copy_ops also performs the copy onto the file system, from the arena
 MKHOST_MATERIALIZE_CHOWN = 16
 MKHOST_UNTAR = 32         # UpdateFromTarReader(untar=true): also write the members under the root
+MKHOST_GUNZIP = 64        # update_from_tar: tar_fd carries a gzip blob, decompressed on the GPU
 MKHOST_COPY_CHOWN, MKHOST_COPY_INTERNAL, MKHOST_COPY_PRESERVE_OWNER, MKHOST_COPY_DEFERRED = 1, 2, 4, 8
 
 

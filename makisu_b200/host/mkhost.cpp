@@ -327,6 +327,8 @@ size_t mkhost_memfs_describe_update_from_tar_ex(mkhost_memfs *m, int64_t now_uni
                                                 size_t cap, char *err, size_t errlen)
 {
     try {
+        if (flags & MKHOST_GUNZIP)
+            throw HostError("MKHOST_GUNZIP: the describe functions read uncompressed tars only");
         m->fs.set_now(now_unix);
         std::vector<uint8_t> buf;
         uint8_t tmp[65536];
@@ -363,6 +365,12 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
         ck(eng, mksnap_begin(eng), "begin");
         const bool file_digests = (flags & MKHOST_FILE_DIGESTS) != 0;
         ArenaTarSource src(eng, tar_fd, want_digest, file_digests);
+        GunzipSession gz;
+        if (flags & MKHOST_GUNZIP) {
+            const std::vector<uint8_t> blob = read_all(tar_fd);
+            gz.open(eng, blob);
+            src.gunzip = eng;
+        }
         const bool untar = (flags & MKHOST_UNTAR) != 0;
         src.allow_split = !untar; // untarOneItem writes a member from one contiguous body
         MemFS::Untar u;
