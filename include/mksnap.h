@@ -282,13 +282,16 @@ int mksnap_get_cdc(const mksnap_t *h, mksnap_cdc_params *out);
  * Independent of begin / finish: a gunzip may be open while an ingest session on the same handle is, so the host can
  * feed the decompressed stream into arenas; calls are serialised by the caller as everywhere else.  One gunzip per
  * handle at a time (open on an open one: MKSNAP_E_STATE).
- * Device memory is allocated at open and freed at close / destroy: the blob and its candidate tables (<= 11 * gz_len),
- * plus one output window of max(256 MiB, largest segment) at 3 bytes per output byte, and a pinned host copy of the
- * window (reads are host copies; one D2H per window).  A blob without flush points is one segment per member, so there
- * the window is as large as the largest member.  Blobs of 16 GiB or more are refused (MKSNAP_E_CAPACITY).  Only the
- * first member body is a scanned start: each later member's first segment is decoded when the link reaches it, one
- * device launch per member.  The gunzip runs on a stream of its own, so window decodes do not wait behind the work of
- * an open session.
+ * Every member body start is a scanned candidate, found on the device at each `1f 8b 08` whose header parses, so the
+ * members of a bgzip / BGZF, eStargz or concatenated blob decode in parallel like the blocks of a pgzip blob.
+ * Device memory is allocated at open and freed at close / destroy: the blob and its candidate tables (at most
+ * gz_len / 4 + gz_len / 3 + 1 candidates at 40 bytes each, <= 25 * gz_len with the blob; a gz_len / 8 bitmap during
+ * the scan only), plus one output window of max(256 MiB, largest segment) at 3 bytes per output byte, and a pinned host
+ * copy of the window (reads are host copies; one D2H per window).  A single member without flush points is one
+ * segment, so there the window is as large as the member, and it decodes on one GPU thread.  Blobs of 16 GiB or more,
+ * and blobs whose candidates do not fit the 32-bit candidate scan, are refused (MKSNAP_E_CAPACITY); candidate tables
+ * that do not fit in device memory fail with MKSNAP_E_NOMEM.  The gunzip runs on a stream of its own, so window
+ * decodes do not wait behind the work of an open session.
  * Acceptance is that of Go's compress/gzip in multistream mode: zlib's inflate for the DEFLATE data; FNAME / FCOMMENT
  * at most 511 bytes; FHCRC checked; whatever follows a member must be another member header (trailing garbage and zero
  * padding are errors).  Malformed headers or DEFLATE data fail open with MKSNAP_E_DATA; a distance before the start of

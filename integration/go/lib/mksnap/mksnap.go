@@ -22,6 +22,7 @@ import "C"
 
 import (
 	"bytes"
+	"compress/gzip"
 	"encoding/hex"
 	"fmt"
 	"io"
@@ -252,17 +253,33 @@ func (fs *MemFS) CommitLayers(e *Engine, now int64, layers [][]CopyOp, tarOuts [
 	return res, nil
 }
 
-// HasFlushPoints reports whether the gzip blob in f carries a flush marker (00 00 FF FF, the empty stored block pgzip
-// ends every 1 MiB block with) in its first 2 MiB: the blobs makisu writes itself (tario.NewGzipWriter) do once they
-// hold more than one block; gzip-CLI and most registry layers never do.  Only such blobs decode in parallel on the
-// device (UpdateFromTar with Gunzip); any other blob is one GPU thread's work.  f is left at offset 0.
-func HasFlushPoints(f *os.File) (bool, error) {
+// DecodesInParallel reports whether the gzip blob in f has, in its first 2 MiB, segment starts that let the device
+// decode it in parallel (UpdateFromTar with Gunzip): a flush marker (00 00 FF FF, the empty stored block pgzip ends
+// every 1 MiB block with: the layers makisu writes itself, tario.NewGzipWriter), or a second member right after the
+// first one's trailer (bgzip / BGZF, eStargz layers, pigz --independent, concatenated gzip files).  A single member
+// without flush points (the gzip CLI, compress/gzip, most registry layers) reports false: it is one GPU thread's work.
+// The first member is inflated on the CPU to find its end, reading at most the 2 MiB.  f is left at offset 0.
+func DecodesInParallel(f *os.File) (bool, error) {
 	buf := make([]byte, 2<<20)
 	n, err := f.ReadAt(buf, 0)
 	if err != nil && err != io.EOF {
 		return false, err
 	}
-	return bytes.Contains(buf[:n], []byte{0, 0, 0xFF, 0xFF}), nil
+	buf = buf[:n]
+	if bytes.Contains(buf, []byte{0, 0, 0xFF, 0xFF}) {
+		return true, nil
+	}
+	br := bytes.NewReader(buf) // an io.ByteReader: the gzip reader takes no byte past the first member's trailer
+	zr, err := gzip.NewReader(br)
+	if err != nil {
+		return false, nil
+	}
+	zr.Multistream(false)
+	if _, err := io.Copy(io.Discard, zr); err != nil {
+		return false, nil // the first member runs past 2 MiB, or is malformed
+	}
+	rest := buf[n-br.Len():]
+	return len(rest) >= 3 && rest[0] == 0x1f && rest[1] == 0x8b && rest[2] == 8, nil
 }
 
 // UpdateFromTar = MemFS.UpdateFromTarReader (mem_fs.go:165-255) on a tar stream, uncompressed or, with Gunzip, the

@@ -1,7 +1,9 @@
 // mksnap_inflate.cuh -- gunzip on the device (mksnap_gunzip_open / _read / _close / _get_times), included at the end of
 // mksnap.cu (the entry points have C linkage through include/mksnap.h).
 //
-//   K5a k_gz_scan_count / k_gz_scan_write  candidate segment starts: the byte after every 00 00 FF FF   (HBM, tiny)
+//   K5a k_gz_scan_headers                  member body starts into a bitmap (one bit per blob byte)   (HBM, tiny)
+//       k_gz_scan_count / k_gz_scan_write  candidate segment starts in offset order: the byte after every
+//                                          00 00 FF FF, and every body start of the bitmap            (HBM, tiny)
 //   K5b k_gz_decode     count mode: speculative decode of every candidate, no output;                 (latency bound)
 //                       write mode: the true segments of one window, 16-bit symbols
 //   K5c k_gz_resolve    window tails in segment order, one CTA                                        (latency, small)
@@ -10,17 +12,19 @@
 //
 // The DEFLATE and gzip logic is mksnap_inflate_core.h (shared with the CPU mock of the engine).  The link -- following
 // the segment ends from each member start, reading trailers and the next member header -- runs on the host over the
-// count results; a start whose count decode was cut short by the K limit, or a later member's body start, is decoded
-// again on the device without the limit, one such start per launch.
+// count results.  Every member body start is a scanned candidate (the scan accepts any header the link accepts), so the
+// members of a bgzip / eStargz / concatenated blob are count-decoded in parallel like flush segments; only a start whose
+// count decode was cut short by the K limit is decoded again on the device without the limit, one such start per
+// launch.  The link treats both kinds of candidate alike: a block that ends on either is a block boundary.
 //
 // Device memory of an open gunzip: the blob (gz_len), 8 bytes per candidate start and 32 per count result (at most
-// gz_len / 4 + 1 candidates: the 00 00 FF FF pattern cannot overlap itself), the segment and extent tables, two 32 KiB
-// history buffers, and one output window of max(GZ_WINDOW, largest segment) bytes at 3 bytes per output byte (16-bit
-// symbols plus bytes), copied once per window to a pinned host buffer of the same size that the reads copy from.  It
-// does not grow with the decompressed length except through the largest segment: a member without flush points is one
-// segment.  Only the first member's body start is scanned; a later member's start is known once the link has read the
-// previous trailer, so its first segment is one of the single-start launches above.  Everything runs on the gunzip's
-// own stream: reads interleaved with an ingest session do not queue behind its kernels.
+// gz_len / 4 + gz_len / 3 + 1 candidates: 00 00 FF FF cannot overlap itself, 1f 8b 08 cannot overlap itself or it, and
+// each header start gives one body start), a bitmap of gz_len / 8 bytes during the scan only, the segment and extent
+// tables, two 32 KiB history buffers, and one output window of max(GZ_WINDOW, largest segment) bytes at 3 bytes per
+// output byte (16-bit symbols plus bytes), copied once per window to a pinned host buffer of the same size that the
+// reads copy from.  It does not grow with the decompressed length except through the largest segment: a member without
+// flush points is one segment.  Everything runs on the gunzip's own stream: reads interleaved with an ingest session
+// do not queue behind its kernels.
 #include "mksnap_inflate_core.h"
 
 namespace gz {
@@ -29,22 +33,51 @@ constexpr uint64_t GZ_WINDOW = 256ull << 20;  // output bytes per window (at lea
 constexpr uint32_t SCAN_CHUNK = 4096;          // blob bytes per scan thread
 constexpr int DEC_WARPS = 2;                   // warps per CTA of k_gz_decode (one segment per warp)
 
-__global__ void k_gz_scan_count(const uint8_t *__restrict__ gz, uint64_t from, uint64_t to, uint32_t *__restrict__ cnt,
-                                uint32_t n_chunks)
+// Member headers: thread c parses every header that starts in [c * SCAN_CHUNK, (c + 1) * SCAN_CHUNK), reading past
+// its chunk as far as the header goes, and sets bit p of `body` for its body start p (from < p <= gz_len).  Body
+// starts are neither ordered nor distinct across header starts, so they meet in a bitmap, and the two kernels below
+// read them back in offset order.
+__global__ void k_gz_scan_headers(const uint8_t *__restrict__ gz, uint64_t gz_len, uint64_t from,
+                                  uint32_t *__restrict__ body, uint32_t n_chunks)
 {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n_chunks)
         return;
-    // candidate p (from < p <= to): gz[p-4..p) == 00 00 FF FF
+    const uint64_t a = (uint64_t)c * SCAN_CHUNK, b = min(a + SCAN_CHUNK, gz_len);
+    for (uint64_t q = a; q < b; ++q) {
+        if (gz[q] != 0x1f)
+            continue;
+        const int64_t p = mki::member_body(gz, gz_len, q);
+        if (p > (int64_t)from)
+            atomicOr(body + (p >> 5), 1u << (p & 31));
+    }
+}
+
+__device__ __forceinline__ bool is_cand(const uint8_t *__restrict__ gz, const uint32_t *__restrict__ body, uint64_t p)
+{
+    return mki::flush_end(gz, p) || ((body[p >> 5] >> (p & 31)) & 1u);
+}
+
+// candidates p, from < p <= to, per chunk: counts (and their sum in *total, to catch a 32-bit scan overflow), then
+// the offsets in order
+__global__ void k_gz_scan_count(const uint8_t *__restrict__ gz, uint64_t from, uint64_t to,
+                                const uint32_t *__restrict__ body, uint32_t *__restrict__ cnt, uint32_t n_chunks,
+                                unsigned long long *__restrict__ total)
+{
+    const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_chunks)
+        return;
     const uint64_t a = from + 1 + (uint64_t)c * SCAN_CHUNK, b = min(a + SCAN_CHUNK, to + 1);
     uint32_t k = 0;
     for (uint64_t p = a; p < b; ++p)
-        k += p >= 4 && gz[p - 1] == 0xFF && gz[p - 2] == 0xFF && gz[p - 3] == 0 && gz[p - 4] == 0;
+        k += is_cand(gz, body, p);
     cnt[c] = k;
+    atomicAdd(total, (unsigned long long)k);
 }
 
 __global__ void k_gz_scan_write(const uint8_t *__restrict__ gz, uint64_t from, uint64_t to,
-                                const uint32_t *__restrict__ base, uint32_t n_chunks, uint64_t *__restrict__ cand)
+                                const uint32_t *__restrict__ body, const uint32_t *__restrict__ base, uint32_t n_chunks,
+                                uint64_t *__restrict__ cand)
 {
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= n_chunks)
@@ -52,7 +85,7 @@ __global__ void k_gz_scan_write(const uint8_t *__restrict__ gz, uint64_t from, u
     const uint64_t a = from + 1 + (uint64_t)c * SCAN_CHUNK, b = min(a + SCAN_CHUNK, to + 1);
     uint64_t *o = cand + 1 + base[c]; // cand[0] is the first member's body start
     for (uint64_t p = a; p < b; ++p)
-        if (p >= 4 && gz[p - 1] == 0xFF && gz[p - 2] == 0xFF && gz[p - 3] == 0 && gz[p - 4] == 0)
+        if (is_cand(gz, body, p))
             *o++ = p;
 }
 
@@ -195,7 +228,8 @@ struct DevScratch {
 // the body of mksnap_gunzip_open; on failure the caller frees the state
 int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_len, mksnap_gunzip_info *info)
 {
-    // candidate counts and their scan are 32-bit: at most gz_len / 4 + 1 candidates
+    // candidate counts and their scan are 32-bit: flush points alone are at most gz_len / 4 + 1; a blob whose member
+    // headers push the total past that is refused after the count (MKSNAP_E_CAPACITY)
     if (gz_len / 4 + 2 > 0xFFFFFFFFull)
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob of %llu bytes exceeds the 16 GiB limit", (unsigned long long)gz_len);
     CK(h, cudaStreamCreateWithFlags(&g->s, cudaStreamNonBlocking));
@@ -218,14 +252,23 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     const uint64_t n_chunks = (to - from + gz::SCAN_CHUNK - 1) / gz::SCAN_CHUNK;
     if (n_chunks > 0xFFFFFFF0ull)
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob too large");
-    DevScratch cnt;
+    const uint64_t n_hchunks = (gz_len + gz::SCAN_CHUNK - 1) / gz::SCAN_CHUNK, body_words = gz_len / 32 + 1;
+    DevScratch cnt, body, tot; // tot: the 64-bit candidate total
     CK(h, cudaMalloc(&cnt.p, (n_chunks + 1) * 4));
-    uint32_t *const d_cnt = (uint32_t *)cnt.p;
+    CK(h, cudaMalloc(&body.p, body_words * 4));
+    CK(h, cudaMalloc(&tot.p, 8));
+    uint32_t *const d_cnt = (uint32_t *)cnt.p, *const d_body = (uint32_t *)body.p;
+    unsigned long long *const d_tot = (unsigned long long *)tot.p;
     CK(h, cudaMemsetAsync(d_cnt, 0, (n_chunks + 1) * 4, s));
+    CK(h, cudaMemsetAsync(d_body, 0, body_words * 4, s));
+    CK(h, cudaMemsetAsync(d_tot, 0, 8, s));
     CK(h, cudaEventRecord(g->ev[0], s));
     const uint32_t tb = 256, nb = (uint32_t)((n_chunks + tb - 1) / tb);
     if (n_chunks) {
-        gz::k_gz_scan_count<<<nb, tb, 0, s>>>(g->d_gz, from, to, d_cnt, (uint32_t)n_chunks);
+        gz::k_gz_scan_headers<<<(uint32_t)((n_hchunks + tb - 1) / tb), tb, 0, s>>>(g->d_gz, gz_len, from, d_body,
+                                                                                  (uint32_t)n_hchunks);
+        LAUNCH_OK(h);
+        gz::k_gz_scan_count<<<nb, tb, 0, s>>>(g->d_gz, from, to, d_body, d_cnt, (uint32_t)n_chunks, d_tot);
         LAUNCH_OK(h);
     }
     // exclusive scan over n_chunks + 1 entries: the last one is the total
@@ -241,14 +284,18 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob too large for the scan scratch of this handle");
     int rc = scan_u32(h, d_cnt, d_cnt, n_chunks + 1, s);
     uint32_t total = 0;
+    unsigned long long total64 = 0;
     if (rc == 0 && cudaMemcpyAsync(&total, d_cnt + n_chunks, 4, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
+        cudaMemcpyAsync(&total64, d_tot, 8, cudaMemcpyDeviceToHost, s) == cudaSuccess &&
         cudaStreamSynchronize(s) == cudaSuccess) {
         g->n_cand = (uint64_t)total + 1;
-        if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess ||
-            cudaMemcpyAsync(g->d_cand, &st.pos, 8, cudaMemcpyHostToDevice, s) != cudaSuccess)
+        if (total64 != total || total64 + 2 > 0xFFFFFFFFull)
+            rc = fail(h, MKSNAP_E_CAPACITY, "gunzip: %llu candidate starts exceed the 32-bit candidate scan", total64);
+        else if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess ||
+                 cudaMemcpyAsync(g->d_cand, &st.pos, 8, cudaMemcpyHostToDevice, s) != cudaSuccess)
             rc = fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
         else if (n_chunks) {
-            gz::k_gz_scan_write<<<nb, tb, 0, s>>>(g->d_gz, from, to, d_cnt, (uint32_t)n_chunks, g->d_cand);
+            gz::k_gz_scan_write<<<nb, tb, 0, s>>>(g->d_gz, from, to, d_body, d_cnt, (uint32_t)n_chunks, g->d_cand);
             h->stats.kernel_launches++;
         }
     } else if (rc == 0) {
@@ -258,6 +305,8 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     if (rc)
         return rc;
     CK(h, cudaGetLastError());
+    CK(h, cudaFree(body.p)); // the bitmap is not needed past the scan: keep it out of the count pass's peak
+    body.p = nullptr;
     CK(h, cudaEventRecord(g->ev[1], s));
 
     // K5b count mode over every candidate

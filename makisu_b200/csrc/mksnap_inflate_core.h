@@ -1,11 +1,15 @@
 // mksnap_inflate_core.h -- the gzip / DEFLATE logic of the engine's gunzip (mksnap_gunzip_*), written once as
 // __host__ __device__ code: the kernels of mksnap_inflate.cuh run it on the H100, the engine's host side runs the link
-// step, and the CPU mock of the engine (tests/mock_engine/mock_mksnap_gunzip.cpp) compiles the same file with g++, so
-// the CPU tests fuzz the code that runs on the GPU.
+// step, and the CPU mock of the engine (tests/mock_engine/mock_mksnap_gunzip_members.cpp, the full candidate rule;
+// mock_mksnap_gunzip.cpp, flush points only) compiles the same file with g++, so the CPU tests fuzz the code that runs
+// on the GPU.
 //
-// Segments.  A blob is cut at candidate starts: the byte after every `00 00 FF FF` (the empty stored block a sync or
-// full flush ends with) and the start of every member body.  decode_segment() decodes from one start until a block
-// ends exactly on a later candidate, or the final block of the member ends.  Decoding from a start that is really a
+// Segments.  A blob is cut at candidate starts (CAND_FLUSH, CAND_MEMBER below): the byte after every `00 00 FF FF` (the empty stored block
+// a sync or full flush ends with) and the body start of every byte-aligned member header the parser accepts, so that
+// the members of a bgzip / eStargz / concatenated blob decode in parallel.  decode_segment() decodes from one start
+// until a block ends exactly on a later candidate, or the final block of the member ends.  A candidate that is not a
+// true start (a pattern inside compressed data) is harmless: decoding from it fails or is never linked, and a block
+// that happens to end on it is a true block boundary, where cutting a segment is exact.  Decoding from a start that is really a
 // block boundary is exact without the output before it, except for back-references into the 32 KiB before the
 // segment: in write mode those bytes become markers (0x8000 | index into that 32 KiB), which resolve_segment_tail()
 // and resolve_symbol() replace once the previous segments are known.
@@ -397,7 +401,9 @@ MKI_HD inline uint32_t crc32_update(uint32_t c, const uint8_t *p, uint64_t n) //
 }
 
 // Member header at `off`: returns the offset of the member body, or -1 (not a valid header, or it is cut short).
-MKI_HD inline int64_t parse_header(const uint8_t *gz, uint64_t gz_len, uint64_t off)
+// check_hcrc = false skips the FHCRC comparison (the two bytes are still required): the candidate scan, where a header
+// with FEXTRA would otherwise cost a bitwise CRC over up to 64 KiB at each of up to gz_len / 3 offsets.
+MKI_HD inline int64_t parse_header(const uint8_t *gz, uint64_t gz_len, uint64_t off, bool check_hcrc = true)
 {
     if (off + 10 > gz_len || gz[off] != 0x1f || gz[off + 1] != 0x8b || gz[off + 2] != 8)
         return -1;
@@ -428,11 +434,34 @@ MKI_HD inline int64_t parse_header(const uint8_t *gz, uint64_t gz_len, uint64_t 
         if (p + 2 > gz_len)
             return -1;
         const uint32_t want = gz[p] | ((uint32_t)gz[p + 1] << 8);
-        if ((crc32_update(0, gz + off, p - off) & 0xFFFFu) != want)
+        if (check_hcrc && (crc32_update(0, gz + off, p - off) & 0xFFFFu) != want)
             return -1;
         p += 2;
     }
     return (int64_t)p;
+}
+
+// ---- candidate starts -----------------------------------------------------------------------------------------------
+// Candidates are the offsets p, first_body < p <= gz_len, of either kind (both bits when both hold); first_body, the
+// first member's body start, is candidate 0.  At most gz_len / 4 + gz_len / 3 + 1 of them: `00 00 FF FF` cannot
+// overlap itself and `1f 8b 08` cannot overlap itself or it, and each header start gives one body start.
+enum : uint8_t {
+    CAND_FLUSH = 1,  // gz[p-4..p) == 00 00 FF FF
+    CAND_MEMBER = 2, // p is the body start of a header at some q < p (member_body(q) == p)
+};
+
+MKI_HD inline bool flush_end(const uint8_t *gz, uint64_t p)
+{
+    return p >= 4 && gz[p - 1] == 0xFF && gz[p - 2] == 0xFF && gz[p - 3] == 0 && gz[p - 4] == 0;
+}
+
+// body start of a member header at q as the scan sees it (FHCRC not compared, see parse_header), or -1.  Bodies of
+// headers at different q need not be in the order of q (FEXTRA can hold a header), nor distinct.
+MKI_HD inline int64_t member_body(const uint8_t *gz, uint64_t gz_len, uint64_t q)
+{
+    if (q + 3 > gz_len || gz[q] != 0x1f || gz[q + 1] != 0x8b || gz[q + 2] != 8)
+        return -1;
+    return parse_header(gz, gz_len, q, false);
 }
 
 // ---- link: the true chain of segments through the speculative results --------------------------------------------
