@@ -52,10 +52,13 @@ enum {
 typedef struct mksnap mksnap_t;
 
 /* Content-defined chunking parameters (DESIGN.md section 3; no reference counterpart). */
+/* Largest max_size mksnap_create accepts: the big-file cut selection works in 16 MiB windows of 32-bit offsets and
+ * computes (offset <= 16 MiB) + max_size, which must not wrap. */
+#define MKSNAP_CDC_MAX_SIZE_LIMIT 0xFEFFFFFFu /* 2^32 - 2^24 - 1 */
 typedef struct {
     uint32_t min_size;    /* default 4096   (must be >= 64)                     */
     uint32_t normal_size; /* default 16384  (strict mask below, loose at/after) */
-    uint32_t max_size;    /* default 131072                                     */
+    uint32_t max_size;    /* default 131072 (at most MKSNAP_CDC_MAX_SIZE_LIMIT)  */
     uint32_t strict_bits; /* default 16: candidate iff the top bits of roll32 are all ones */
     uint32_t loose_bits;  /* default 12                                         */
 } mksnap_cdc_params;

@@ -630,6 +630,9 @@ static int create_impl(mksnap *h)
     return 0;
 }
 
+// sel_rule: a window offset (at most the window, SELB_REGIONS regions) plus max_size stays a 32-bit value
+static_assert((uint64_t)SELB_REGIONS * SCAN_TILE + MKSNAP_CDC_MAX_SIZE_LIMIT <= 0xFFFFFFFFull, "max_size limit");
+
 int mksnap_create(const mksnap_config *cfg, mksnap_t **out)
 {
     if (!cfg || !out)
@@ -641,8 +644,8 @@ int mksnap_create(const mksnap_config *cfg, mksnap_t **out)
     if (p.min_size == 0 && p.max_size == 0)
         mksnap_default_cdc(&p);
     h->cfg.cdc = p;
-    if (p.min_size < 64 || p.normal_size < p.min_size || p.max_size < p.normal_size || p.strict_bits < p.loose_bits ||
-        p.strict_bits > 31 || p.loose_bits < 1) {
+    if (p.min_size < 64 || p.normal_size < p.min_size || p.max_size < p.normal_size ||
+        p.max_size > MKSNAP_CDC_MAX_SIZE_LIMIT || p.strict_bits < p.loose_bits || p.strict_bits > 31 || p.loose_bits < 1) {
         g_create_error = "invalid cdc parameters";
         delete h;
         return MKSNAP_E_INVAL;

@@ -978,7 +978,11 @@ k_select_cuts_big(const CdcFile *__restrict__ files, uint32_t n_files, CdcParams
         w.ncand = s_off[nreg];
         w.wend = nreg * SCAN_TILE;
         // a piece whose file continues (more_after) has no file end in sight: the chain stops with NX_OUT near the
-        // piece end and the exact rule (select_one_cut with more_after) finishes from global memory
+        // piece end and the exact rule (select_one_cut with more_after) finishes from global memory.  Its window ends
+        // at the piece end, not at the end of the piece's last region: bytes behind the piece are not the file's, and
+        // neither a forced cut nor a candidate there may end a chunk.
+        if (fl.more_after && wbase + w.wend > end)
+            w.wend = (uint32_t)(end - wbase);
         w.fend = (wbase + w.wend >= end && !fl.more_after) ? (uint32_t)(end - wbase) : 0xFFFFFFFFu;
         // ---- 2. next[] for every candidate, in parallel ----
         for (uint32_t q = threadIdx.x; q < w.ncand; q += SELB_THREADS) {
