@@ -104,8 +104,11 @@ typedef struct {
  * lib/builder/step/common.go:44-55: every tar.Writer write lands in one stream).  arena_off multiple of 16.
  * `stream` is a caller-chosen slot in [0, max_extents): the digest of the stream lands in row `stream` of the
  * stream-digest table.  A stream may span several submits (a layer tar larger than one arena): every piece but
- * the last carries MKSNAP_R_MORE and a length that is a multiple of 64; the device keeps the SHA-256 midstate
- * between submits.  At most one piece per stream per submit. */
+ * the last carries MKSNAP_R_MORE and a length that is a non-empty multiple of 64; the device keeps the SHA-256
+ * midstate between submits.  The last piece may be empty (every byte went out in earlier pieces).  At most one piece
+ * per stream per submit.  mksnap_finish refuses a session whose stream is still open (its last piece carried
+ * MKSNAP_R_MORE) with MKSNAP_E_STATE; the session stays open, so the final piece can still be submitted.  A slot may
+ * carry a new stream once its previous stream has finished. */
 #define MKSNAP_R_MORE 1u
 typedef struct {
     uint64_t arena_off;
@@ -325,7 +328,8 @@ int mksnap_get_table(mksnap_t *h, uint8_t *table, uint64_t capacity_rows);
 /* rows the handle's table currently holds: result.n_unique after finish / allgather, this rank's range after exchange */
 uint64_t mksnap_table_rows(mksnap_t *h);
 /* stream digests, row = stream slot: the TarDigest bytes of
- * lib/builder/step/common.go:86 (hex-encode and prefix "sha256:" on the host). */
+ * lib/builder/step/common.go:86 (hex-encode and prefix "sha256:" on the host).  Rows [0, result.n_streams); the row of
+ * a slot on which no stream finished in the session is unspecified (it may hold an earlier session's digest). */
 int mksnap_get_stream_digests(mksnap_t *h, uint8_t *digests, uint64_t capacity);
 
 /* ---- multi-GPU: one process per GPU, files sharded, one exchange step ---- */

@@ -121,6 +121,8 @@ struct mksnap {
     StreamState *d_stream_state = nullptr;
     std::vector<uint32_t> stream_stamp; // submit epoch that last used the stream slot (one piece per stream per submit)
     uint32_t stamp_epoch = 0;
+    std::vector<uint8_t> stream_open; // per slot: the last piece carried MKSNAP_R_MORE (finish refuses the session)
+    uint64_t n_open = 0;              // slots with stream_open set
     uint64_t n_streams = 0;
     uint64_t stream_base = 0; // bytes of arenas submitted before the current one
     uint64_t crc_bytes = 0;
@@ -609,6 +611,7 @@ static int create_impl(mksnap *h)
     CK(h, cudaMalloc(&h->d_stream_state, h->max_streams * sizeof(StreamState)));
     CK(h, cudaMemset(h->d_stream_state, 0, h->max_streams * sizeof(StreamState)));
     h->stream_stamp.assign(h->max_streams, 0);
+    h->stream_open.assign(h->max_streams, 0);
 
     {
         int rc = alloc_table_buffers(h, mc);
@@ -741,6 +744,10 @@ int mksnap_begin(mksnap_t *h)
     h->crc_host_acc = 0;
     h->crc_host_bytes = 0;
     h->open_file = false;
+    if (h->n_open) {
+        std::fill(h->stream_open.begin(), h->stream_open.end(), 0);
+        h->n_open = 0;
+    }
     h->n_unique = 0;
     h->finished = false;
     h->in_session = true;
@@ -1053,9 +1060,17 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
     m.in_flight = true;
     h->slot_used[slot] = true;
     h->have_submit_times = true;
-    for (uint64_t i = 0; i < n_rng; i++)
-        if (!(rng[i].flags & MKSNAP_R_MORE))
+    for (uint64_t i = 0; i < n_rng; i++) {
+        const bool more = (rng[i].flags & MKSNAP_R_MORE) != 0;
+        uint8_t &open = h->stream_open[rng[i].stream];
+        if (more && !open)
+            h->n_open++;
+        else if (!more && open)
+            h->n_open--;
+        open = more;
+        if (!more)
             h->n_streams = std::max<uint64_t>(h->n_streams, (uint64_t)rng[i].stream + 1);
+    }
     h->open_file = have_more;
     h->stream_base += used;
     h->crc_bytes += crc_bytes;
@@ -1243,6 +1258,9 @@ int mksnap_finish(mksnap_t *h, mksnap_result *out)
         return fail(h, MKSNAP_E_STATE, "internal: open chunk of a continued file exceeds the carry buffer");
     if (h->open_file)
         return fail(h, MKSNAP_E_STATE, "finish: the last submit left a file open (MKSNAP_X_MORE without its continuation)");
+    if (h->n_open)
+        return fail(h, MKSNAP_E_STATE, "finish: %llu stream(s) left open (last piece carried MKSNAP_R_MORE)",
+                    (unsigned long long)h->n_open);
     if (h->h_sc->err & 2u)
         return fail(h, MKSNAP_E_CAPACITY, "chunk table overflow (max_chunks = %llu)", (unsigned long long)h->max_chunks);
     const uint64_t n = h->h_sc->n_chunks;

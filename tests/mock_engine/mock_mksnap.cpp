@@ -5,7 +5,8 @@
 // the arena) can be exercised without a GPU: tests/test_host_mock_engine_cpu.py loads it with RTLD_GLOBAL *before*
 // libmkhost in a fresh process, so libmkhost's mksnap_* references bind here.  It is never loaded by the product,
 // lives under tests/, and enforces the same contract the real library does (offsets inside `used`, 16-byte aligned
-// ranges, non-final stream pieces in multiples of 64 bytes, one piece per stream per submit, stream slot < max_extents).
+// ranges, non-final stream pieces non-empty multiples of 64 bytes, one piece per stream per submit, stream slot <
+// max_extents, no stream left open at finish).
 #include <stdint.h>
 #include <string.h>
 
@@ -212,16 +213,19 @@ int mksnap_arena_submit(mksnap_t *h, int32_t arena_id, uint64_t used, const mksn
         }
     }
     std::set<uint32_t> seen;
-    for (uint64_t i = 0; i < n_rng; ++i) {
+    for (uint64_t i = 0; i < n_rng; ++i) { // every range is checked before any stream moves, as on the engine
         const mksnap_range &r = rng[i];
         if (r.arena_off % 16 || r.arena_off + r.len > used)
             return fail(h, MKSNAP_E_INVAL, "range outside the submitted bytes or not 16-byte aligned");
         if (r.stream >= h->cfg.max_extents)
             return fail(h, MKSNAP_E_CAPACITY, "stream slot beyond max_extents");
+        if ((r.flags & MKSNAP_R_MORE) && (r.len == 0 || r.len % 64))
+            return fail(h, MKSNAP_E_INVAL, "non-final stream piece is empty or not a multiple of 64 bytes");
         if (!seen.insert(r.stream).second)
             return fail(h, MKSNAP_E_INVAL, "two pieces of one stream in one submit");
-        if ((r.flags & MKSNAP_R_MORE) && r.len % 64)
-            return fail(h, MKSNAP_E_INVAL, "non-final stream piece is not a multiple of 64 bytes");
+    }
+    for (uint64_t i = 0; i < n_rng; ++i) {
+        const mksnap_range &r = rng[i];
         auto it = h->open_streams.find(r.stream);
         if (it == h->open_streams.end()) {
             mko_sha256_ctx c;
