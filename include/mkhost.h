@@ -250,6 +250,26 @@ size_t mkhost_memfs_describe_update_from_tar(mkhost_memfs *m, int64_t now_unix, 
 size_t mkhost_memfs_describe_update_from_tar_ex(mkhost_memfs *m, int64_t now_unix, int tar_fd, uint32_t flags, char *out,
                                                 size_t cap, char *err, size_t errlen);
 
+/* A run of layers applied back to back in ONE engine session (FromStep.Execute merging the layers of the base image,
+ * from_step.go:118-134; buildNode.Build applying the layers of cached steps, build_node.go:72-79,133-148).  The result
+ * equals n_layers calls of mkhost_memfs_update_from_tar in order: the same tree, the same files on disk under
+ * MKHOST_UNTAR, the same remembered file digests, and per layer the same outs[i].tar_digest, n_entries and tar_bytes;
+ * outs[i].root / n_chunks / n_unique describe the chunk table of the whole run (one session).  The layers are read and
+ * merged strictly in order, but their DiffID chains are hashed together: layer i's tar stream is stream slot i, a
+ * MKSNAP_R_DEFER stream, so its bytes wait in the engine's stream log and every chain of the run advances in the same
+ * K4 launches (one chain on an H100 runs at ~0.06 GB/s).  The call reserves the stream log itself (1 GiB) and leaves it
+ * reserved on the handle.  flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS (per-file streams take the slots after
+ * n_layers and stay inline; the engine needs max_extents > n_layers), MKHOST_UNTAR.  layers[i].flags: MKHOST_GUNZIP
+ * for a gzip blob.  The chunks of the whole run share one session's table (mksnap_limits.max_chunks).  A run with
+ * more layers than stream slots fails before anything is read.  If layer k fails, layers
+ * before k stay merged in the tree and on disk, as after separate calls; the call returns -1 and outs is unspecified. */
+typedef struct {
+    int tar_fd;
+    uint32_t flags; /* MKHOST_GUNZIP: this blob is gzip */
+} mkhost_tar_spec;
+int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
+                                  size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen);
+
 /* CopyOperation.Execute (lib/snapshot/copy_op.go:82-147) with fileio.Copier (lib/fileio/copy.go): what a COPY/ADD step
  * does to the file system when it runs with --modifyfs.  op->dst is used as the on-disk destination exactly like the
  * reference does (resolved against op->work_dir when relative).  mode selects the Copier of copy_op.go:98-124:

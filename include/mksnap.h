@@ -110,6 +110,17 @@ typedef struct {
  * MKSNAP_R_MORE) with MKSNAP_E_STATE; the session stays open, so the final piece can still be submitted.  A slot may
  * carry a new stream once its previous stream has finished. */
 #define MKSNAP_R_MORE 1u
+/* A piece of a DEFERRED stream: its bytes are copied on the device from the arena slot into the handle's stream log
+ * (mksnap_reserve_stream_log) before the slot is recycled, and hashed later, together with the deferred pieces of every
+ * other stream, so that many chains advance in the same K4 launch even when the caller fills arenas one stream after
+ * the other (layers applied in order).  The log is hashed ("flushed") at mksnap_finish at the latest, and earlier when
+ * a deferred piece does not fit in the room left: the pending pieces are grouped by stream in log order, adjacent
+ * pieces of one stream merged, and K4 runs once per round (the r-th remaining piece of every stream).  A deferred piece
+ * larger than the whole log, and every deferred piece of a handle without a log, is hashed in its own submit.
+ * Every other rule of this table is unchanged and digests are bit-identical to the inline path.  All pieces of one
+ * stream carry the flag or none does (MKSNAP_E_INVAL otherwise); deferred and inline streams may share a session.
+ * The row of a deferred stream is readable after mksnap_finish only. */
+#define MKSNAP_R_DEFER 2u
 typedef struct {
     uint64_t arena_off;
     uint64_t len;
@@ -145,6 +156,7 @@ typedef struct {
     uint64_t kernel_launches; /* kernels launched by this handle since create */
     uint64_t h2d_bytes;       /* since create */
     uint64_t d2h_bytes;       /* since create */
+    float ms_flush;           /* K4 rounds of the most recent stream-log flush (MKSNAP_R_DEFER) */
 } mksnap_stats_t;
 
 /* ---- lifetime --------------------------------------------------------- */
@@ -183,6 +195,12 @@ typedef struct {
     uint64_t carry_bytes;        /* earliest arena offset of a MKSNAP_X_CONT extent (max chunk size, 512-aligned) */
 } mksnap_limits;
 int mksnap_get_limits(const mksnap_t *h, mksnap_limits *out);
+
+/* Device memory for the stream log of MKSNAP_R_DEFER pieces: allocate it, resize it to `bytes` (rounded up to 64), or
+ * free it (bytes == 0).  Refused with MKSNAP_E_STATE while deferred pieces wait in the log (a session between its
+ * first deferred piece and finish); callable outside a session and right after begin.  Each deferred piece takes its
+ * length rounded up to 16 bytes of the log.  The log stays allocated until resized, freed or the handle is destroyed. */
+int mksnap_reserve_stream_log(mksnap_t *h, uint64_t bytes);
 
 /* Async: copy arena[0,used) host->device, then run CRC over MKSNAP_X_CRC
  * extents, CDC + per-chunk SHA-256 over MKSNAP_X_CDC extents and one serial
@@ -329,7 +347,9 @@ int mksnap_get_table(mksnap_t *h, uint8_t *table, uint64_t capacity_rows);
 uint64_t mksnap_table_rows(mksnap_t *h);
 /* stream digests, row = stream slot: the TarDigest bytes of
  * lib/builder/step/common.go:86 (hex-encode and prefix "sha256:" on the host).  Rows [0, result.n_streams); the row of
- * a slot on which no stream finished in the session is unspecified (it may hold an earlier session's digest). */
+ * a slot on which no stream finished in the session is unspecified (it may hold an earlier session's digest).  Inside a
+ * session the call waits for the submits enqueued so far; the row of a stream that finished inline (not MKSNAP_R_DEFER)
+ * in one of them is then final, and the slot may carry a new stream afterwards. */
 int mksnap_get_stream_digests(mksnap_t *h, uint8_t *digests, uint64_t capacity);
 
 /* ---- multi-GPU: one process per GPU, files sharded, one exchange step ---- */

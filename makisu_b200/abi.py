@@ -51,6 +51,7 @@ class Range(C.Structure):
 
 
 MKSNAP_R_MORE = 1
+MKSNAP_R_DEFER = 2  # the piece goes to the handle's stream log and is hashed later with other streams' pieces
 
 
 class CrcUse(C.Structure):
@@ -77,7 +78,7 @@ class Stats(C.Structure):
     _fields_ = [("ms_total", C.c_float), ("ms_crc", C.c_float), ("ms_scan", C.c_float), ("ms_select", C.c_float),
                 ("ms_sha", C.c_float), ("ms_stream", C.c_float), ("ms_h2d", C.c_float), ("ms_sort", C.c_float),
                 ("ms_root", C.c_float), ("ms_gather", C.c_float), ("kernel_launches", C.c_uint64),
-                ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64)]
+                ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64), ("ms_flush", C.c_float)]
 
 
 class Limits(C.Structure):
@@ -107,6 +108,7 @@ SYMBOLS = [
     ("mksnap_arena_acquire", C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_uint64), C.POINTER(C.c_int32)]),
     ("mksnap_arena_release", C.c_int, [_P, C.c_int32]),
     ("mksnap_get_limits", C.c_int, [_P, C.POINTER(Limits)]),
+    ("mksnap_reserve_stream_log", C.c_int, [_P, C.c_uint64]),
     ("mksnap_arena_submit", C.c_int, [_P, C.c_int32, C.c_uint64, C.POINTER(Extent), C.c_uint64, C.POINTER(Range), C.c_uint64]),
     ("mksnap_device_arena", C.c_int, [_P, C.c_uint32, C.POINTER(_P), C.POINTER(C.c_uint64)]),
     ("mksnap_device_upload", C.c_int, [_P, C.c_uint32, C.c_uint64, _P, C.c_uint64]),
@@ -263,6 +265,10 @@ class Engine:
         out = Limits()
         self._ck(self.lib.mksnap_get_limits(self.h, C.byref(out)), "mksnap_get_limits")
         return out
+
+    def reserve_stream_log(self, nbytes: int):
+        """Size the device log that MKSNAP_R_DEFER pieces wait in (0 frees it); outside a session only."""
+        self._ck(self.lib.mksnap_reserve_stream_log(self.h, nbytes), "mksnap_reserve_stream_log")
 
     @staticmethod
     def _tables(extents, ranges):

@@ -15,6 +15,7 @@
 
 #include <algorithm>
 #include <string>
+#include <unordered_map>
 #include <vector>
 
 using namespace mk;
@@ -125,6 +126,20 @@ struct mksnap {
     uint64_t n_open = 0;              // slots with stream_open set
     uint64_t n_streams = 0;
     uint64_t stream_base = 0; // bytes of arenas submitted before the current one
+    // MKSNAP_R_DEFER: the stream log and the pieces waiting in it (log order)
+    std::vector<uint8_t> stream_defer; // per slot: the open stream is a deferred one
+    std::vector<uint32_t> log_count;   // per slot: pieces waiting in the log
+    struct LogPiece {
+        uint64_t off, len;
+        uint32_t stream, more;
+    };
+    std::vector<LogPiece> log_pending;
+    uint8_t *d_log = nullptr;
+    uint64_t log_cap = 0, log_used = 0;
+    uint64_t *h_flush = nullptr, *d_flush = nullptr; // K4 tables of a flush: start, len (u64), stream, flags (u32)
+    uint64_t flush_cap = 0;                          // rows
+    cudaEvent_t ev_flush = nullptr;                  // the last flush's table copy has left h_flush
+    bool have_flush_time = false;
     uint64_t crc_bytes = 0;
     uint32_t *d_crc_session = nullptr; // pure(extent) of every CRC extent of the session, submission order
     uint64_t crc_session_cap = 0, crc_session_n = 0;
@@ -612,6 +627,9 @@ static int create_impl(mksnap *h)
     CK(h, cudaMemset(h->d_stream_state, 0, h->max_streams * sizeof(StreamState)));
     h->stream_stamp.assign(h->max_streams, 0);
     h->stream_open.assign(h->max_streams, 0);
+    h->stream_defer.assign(h->max_streams, 0);
+    h->log_count.assign(h->max_streams, 0);
+    CK(h, cudaEventCreateWithFlags(&h->ev_flush, cudaEventDisableTiming));
 
     {
         int rc = alloc_table_buffers(h, mc);
@@ -713,6 +731,9 @@ void mksnap_destroy(mksnap_t *h)
     cudaFree(h->d_scan_tmp);
     cudaFree(h->d_order); cudaFree(h->d_chunk_start); cudaFree(h->d_chunk_len); cudaFree(h->d_chunk_end); cudaFree(h->d_digests);
     cudaFree(h->d_stream_digests); cudaFree(h->d_stream_state);
+    cudaFree(h->d_log); cudaFree(h->d_flush); cudaFreeHost(h->h_flush);
+    if (h->ev_flush)
+        cudaEventDestroy(h->ev_flush);
     for (int k = 0; k < 2; k++) {
         cudaFree(h->d_keys[k]); cudaFree(h->d_idx[k]); cudaFree(h->d_merkle[k]);
     }
@@ -748,6 +769,10 @@ int mksnap_begin(mksnap_t *h)
         std::fill(h->stream_open.begin(), h->stream_open.end(), 0);
         h->n_open = 0;
     }
+    for (const auto &p : h->log_pending) // pieces of an abandoned session are dropped
+        h->log_count[p.stream] = 0;
+    h->log_pending.clear();
+    h->log_used = 0;
     h->n_unique = 0;
     h->finished = false;
     h->in_session = true;
@@ -813,6 +838,116 @@ static bool in_spans(const mksnap_span *sp, uint64_t n, uint64_t off, uint64_t l
         return true;
     const mksnap_span *it = std::upper_bound(sp, sp + n, off, [](uint64_t v, const mksnap_span &s) { return v < s.off; });
     return it != sp && off + len <= (it - 1)->off + (it - 1)->len;
+}
+
+int mksnap_reserve_stream_log(mksnap_t *h, uint64_t bytes)
+{
+    if (!h)
+        return MKSNAP_E_INVAL;
+    if (!h->log_pending.empty())
+        return fail(h, MKSNAP_E_STATE, "reserve_stream_log while %llu deferred piece(s) wait in the log",
+                    (unsigned long long)h->log_pending.size());
+    CK(h, cudaSetDevice(h->cfg.device));
+    bytes = (bytes + 63) & ~63ull; // K4 reads a piece's last block in whole 16-byte words
+    if (bytes == h->log_cap)
+        return 0;
+    CK(h, cudaStreamSynchronize(h->s_comp));
+    CK(h, cudaFree(h->d_log));
+    h->d_log = nullptr;
+    h->log_cap = 0;
+    if (bytes) {
+        if (cudaMalloc(&h->d_log, bytes) != cudaSuccess) {
+            cudaGetLastError();
+            h->d_log = nullptr;
+            return fail(h, MKSNAP_E_NOMEM, "stream log of %llu bytes", (unsigned long long)bytes);
+        }
+        h->log_cap = bytes;
+    }
+    return 0;
+}
+
+// Hash every piece waiting in the stream log, enqueued on the compute stream.  Pieces are grouped by stream in log
+// order; a piece that continues its stream's previous group (contiguous in the log, or empty) joins it.  Round r is the
+// r-th group of every stream: one K4 launch per round keeps K4's rule of one piece per stream per launch, and a slot
+// that carried two streams hashes them in order (the first group's final piece closes the midstate the second starts
+// from).
+static int flush_log(mksnap *h, cudaStream_t sk)
+{
+    if (h->log_pending.empty()) {
+        h->log_used = 0;
+        return 0;
+    }
+    struct Group {
+        uint64_t off, len;
+        uint32_t stream, more, round;
+    };
+    std::vector<Group> groups;
+    std::vector<uint32_t> per_round;
+    std::unordered_map<uint32_t, int64_t> last; // stream -> its latest group
+    for (const auto &p : h->log_pending) {
+        const auto ins = last.emplace(p.stream, -1);
+        int64_t &g = ins.first->second;
+        if (g >= 0 && groups[g].more && (p.len == 0 || groups[g].off + groups[g].len == p.off)) {
+            groups[g].len += p.len;
+            groups[g].more = p.more;
+            continue;
+        }
+        const uint32_t round = g >= 0 ? groups[g].round + 1 : 0;
+        if (round == per_round.size())
+            per_round.push_back(0);
+        per_round[round]++;
+        g = (int64_t)groups.size();
+        groups.push_back(Group{p.off, p.len, p.stream, p.more, round});
+    }
+    const uint64_t n = groups.size();
+    if (n > h->flush_cap) {
+        CK(h, cudaStreamSynchronize(sk));
+        CK(h, cudaFreeHost(h->h_flush));
+        CK(h, cudaFree(h->d_flush));
+        h->h_flush = h->d_flush = nullptr;
+        h->flush_cap = 0;
+        const uint64_t cap = std::max<uint64_t>(n, 1024);
+        CK(h, cudaHostAlloc(&h->h_flush, cap * 24, cudaHostAllocDefault));
+        CK(h, cudaMalloc(&h->d_flush, cap * 24));
+        h->flush_cap = cap;
+    } else {
+        CK(h, cudaEventSynchronize(h->ev_flush));
+    }
+    // rows ordered by round: [start n][len n][stream n][flags n]
+    std::vector<uint64_t> at(per_round.size(), 0);
+    for (size_t r = 1; r < per_round.size(); r++)
+        at[r] = at[r - 1] + per_round[r - 1];
+    uint64_t *start = h->h_flush, *len = start + n;
+    uint32_t *stream = reinterpret_cast<uint32_t *>(len + n), *flags = stream + n;
+    for (const Group &g : groups) {
+        const uint64_t i = at[g.round]++;
+        start[i] = g.off;
+        len[i] = g.len;
+        stream[i] = g.stream;
+        flags[i] = g.more ? MKSNAP_R_MORE : 0u;
+    }
+    CK(h, cudaMemcpyAsync(h->d_flush, h->h_flush, n * 24, cudaMemcpyHostToDevice, sk));
+    CK(h, cudaEventRecord(h->ev_flush, sk));
+    h->stats.h2d_bytes += n * 24;
+    const uint64_t *d_start = h->d_flush, *d_len = d_start + n;
+    const uint32_t *d_stream = reinterpret_cast<const uint32_t *>(d_len + n), *d_flags = d_stream + n;
+    CK(h, cudaEventRecord(h->ev[6], sk));
+    for (uint64_t r = 0, o = 0; r < per_round.size(); o += per_round[r], r++) {
+        const uint32_t pairs = (uint32_t)((per_round[r] + 31) / 32);
+        CK(h, cudaMemsetAsync(&h->d_sc->work, 0, 4, sk));
+        k_sha256_streams<<<std::min<uint32_t>(pairs, (uint32_t)h->sm_count * 4), SS_THREADS, 0, sk>>>(
+            h->d_log, d_start + o, d_len + o, per_round[r], d_stream + o, d_flags + o, h->d_stream_state,
+            h->d_stream_digests, &h->d_sc->work, 32u, 1u);
+        LAUNCH_OK(h);
+    }
+    CK(h, cudaMemsetAsync(&h->d_sc->work, 0, 4, sk));
+    CK(h, cudaEventRecord(h->ev[7], sk));
+    h->have_flush_time = true;
+    for (const auto &p : h->log_pending)
+        h->log_count[p.stream] = 0;
+    h->log_pending.clear();
+    h->log_used = 0;
+    return 0;
 }
 
 // src != nullptr: the arena comes from that pinned host arena, and of [0, used) only `spans` travel (the rest is zeroed)
@@ -906,11 +1041,25 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         if (h->stream_stamp[rng[i].stream] == h->stamp_epoch)
             return fail(h, MKSNAP_E_INVAL, "range %llu: stream slot %u already has a piece in this submit (one piece per stream per submit)",
                         (unsigned long long)i, rng[i].stream);
+        const bool defer = (rng[i].flags & MKSNAP_R_DEFER) != 0;
+        if (h->stream_open[rng[i].stream] && h->stream_defer[rng[i].stream] != defer)
+            return fail(h, MKSNAP_E_INVAL, "range %llu: stream slot %u mixes MKSNAP_R_DEFER and inline pieces in one stream",
+                        (unsigned long long)i, rng[i].stream);
         h->stream_stamp[rng[i].stream] = h->stamp_epoch;
-        m.h_rstart[i] = rng[i].arena_off;
-        m.h_rlen[i] = rng[i].len;
-        m.h_rstream[i] = rng[i].stream;
-        m.h_rflags[i] = rng[i].flags;
+    }
+    // deferred pieces go to the stream log; the rest (and deferred pieces the log cannot hold) is hashed by this submit
+    std::vector<uint64_t> logged;
+    uint64_t n_inline = 0;
+    for (uint64_t i = 0; i < n_rng; i++) {
+        if ((rng[i].flags & MKSNAP_R_DEFER) && h->log_cap && rng[i].len <= h->log_cap) {
+            logged.push_back(i);
+            continue;
+        }
+        m.h_rstart[n_inline] = rng[i].arena_off;
+        m.h_rlen[n_inline] = rng[i].len;
+        m.h_rstream[n_inline] = rng[i].stream;
+        m.h_rflags[n_inline] = rng[i].flags & MKSNAP_R_MORE;
+        n_inline++;
     }
 
     uint8_t *d_arena = h->d_slot[slot];
@@ -948,13 +1097,13 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
     }
     if (n_files)
         CK(h, cudaMemcpyAsync(m.d_files, m.h_files, n_files * sizeof(CdcFile), cudaMemcpyHostToDevice, sc));
-    if (n_rng) {
-        CK(h, cudaMemcpyAsync(m.d_rstart, m.h_rstart, n_rng * 8, cudaMemcpyHostToDevice, sc));
-        CK(h, cudaMemcpyAsync(m.d_rlen, m.h_rlen, n_rng * 8, cudaMemcpyHostToDevice, sc));
-        CK(h, cudaMemcpyAsync(m.d_rstream, m.h_rstream, n_rng * 4, cudaMemcpyHostToDevice, sc));
-        CK(h, cudaMemcpyAsync(m.d_rflags, m.h_rflags, n_rng * 4, cudaMemcpyHostToDevice, sc));
+    if (n_inline) {
+        CK(h, cudaMemcpyAsync(m.d_rstart, m.h_rstart, n_inline * 8, cudaMemcpyHostToDevice, sc));
+        CK(h, cudaMemcpyAsync(m.d_rlen, m.h_rlen, n_inline * 8, cudaMemcpyHostToDevice, sc));
+        CK(h, cudaMemcpyAsync(m.d_rstream, m.h_rstream, n_inline * 4, cudaMemcpyHostToDevice, sc));
+        CK(h, cudaMemcpyAsync(m.d_rflags, m.h_rflags, n_inline * 4, cudaMemcpyHostToDevice, sc));
     }
-    h->stats.h2d_bytes += n_crc * sizeof(CrcExtent) + (n_crc ? (n_crc + 1) * 4 : 0) + n_files * sizeof(CdcFile) + n_rng * 16;
+    h->stats.h2d_bytes += n_crc * sizeof(CrcExtent) + (n_crc ? (n_crc + 1) * 4 : 0) + n_files * sizeof(CdcFile) + n_inline * 16;
     CK(h, cudaEventRecord(h->ev_copy_done, sc));
 
     // ---- compute stream ----
@@ -1044,12 +1193,35 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         }
     }
     CK(h, cudaEventRecord(h->ev[4], sk));
-    if (n_rng) {
+    for (const uint64_t i : logged) { // into the log before the slot is recycled; a full log is hashed first
+        const mksnap_range &r = rng[i];
+        uint64_t off = (h->log_used + 15) & ~15ull;
+        if (off + r.len > h->log_cap) {
+            int rc = flush_log(h, sk);
+            if (rc)
+                return rc;
+            off = 0;
+        }
+        if (r.len)
+            CK(h, cudaMemcpyAsync(h->d_log + off, d_arena + r.arena_off, r.len, cudaMemcpyDeviceToDevice, sk));
+        h->log_pending.push_back(mksnap::LogPiece{off, r.len, r.stream, r.flags & MKSNAP_R_MORE});
+        h->log_count[r.stream]++;
+        h->log_used = off + r.len;
+    }
+    bool behind_log = false; // an inline piece on a slot whose earlier pieces wait in the log
+    for (uint64_t k = 0; k < n_inline; k++)
+        behind_log |= h->log_count[m.h_rstream[k]] != 0;
+    if (behind_log) {
+        int rc = flush_log(h, sk);
+        if (rc)
+            return rc;
+    }
+    if (n_inline) {
         // K4: warp pairs, 32 streams each, spread one pair per SM first (a pair then owns its two sub-partitions)
         CK(h, cudaMemsetAsync(&h->d_sc->work, 0, 4, sk));
-        const uint32_t pairs = (uint32_t)((n_rng + 31) / 32);
+        const uint32_t pairs = (uint32_t)((n_inline + 31) / 32);
         k_sha256_streams<<<std::min<uint32_t>(pairs, (uint32_t)h->sm_count * 4), SS_THREADS, 0, sk>>>(
-            d_arena, m.d_rstart, m.d_rlen, (uint32_t)n_rng, m.d_rstream, m.d_rflags, h->d_stream_state, h->d_stream_digests,
+            d_arena, m.d_rstart, m.d_rlen, (uint32_t)n_inline, m.d_rstream, m.d_rflags, h->d_stream_state, h->d_stream_digests,
             &h->d_sc->work, 32u, 1u);
         LAUNCH_OK(h);
         CK(h, cudaMemsetAsync(&h->d_sc->work, 0, 4, sk));
@@ -1068,6 +1240,7 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         else if (!more && open)
             h->n_open--;
         open = more;
+        h->stream_defer[rng[i].stream] = (rng[i].flags & MKSNAP_R_DEFER) != 0;
         if (!more)
             h->n_streams = std::max<uint64_t>(h->n_streams, (uint64_t)rng[i].stream + 1);
     }
@@ -1263,9 +1436,12 @@ int mksnap_finish(mksnap_t *h, mksnap_result *out)
                     (unsigned long long)h->n_open);
     if (h->h_sc->err & 2u)
         return fail(h, MKSNAP_E_CAPACITY, "chunk table overflow (max_chunks = %llu)", (unsigned long long)h->max_chunks);
+    int rc = flush_log(h, s);
+    if (rc)
+        return rc;
     const uint64_t n = h->h_sc->n_chunks;
     CK(h, cudaEventRecord(h->ev_fin[0], s));
-    int rc = sort_unique_root(h, h->d_digests, n, s);
+    rc = sort_unique_root(h, h->d_digests, n, s);
     if (rc)
         return rc;
     CK(h, cudaEventRecord(h->ev_fin[1], s));
@@ -1485,6 +1661,8 @@ int mksnap_stats(mksnap_t *h, mksnap_stats_t *out)
         CK(h, cudaEventElapsedTime(&h->stats.ms_sort, h->ev_fin[0], h->ev_fin[1]));
         CK(h, cudaEventElapsedTime(&h->stats.ms_root, h->ev_fin[1], h->ev_fin[2]));
     }
+    if (h->have_flush_time)
+        CK(h, cudaEventElapsedTime(&h->stats.ms_flush, h->ev[6], h->ev[7]));
     *out = h->stats;
     return 0;
 }

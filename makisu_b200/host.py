@@ -44,6 +44,10 @@ class LayerResult(C.Structure):
                 ("tar_bytes", C.c_uint64), ("n_chunks", C.c_uint64), ("n_unique", C.c_uint64)]
 
 
+class TarSpec(C.Structure):
+    _fields_ = [("tar_fd", C.c_int), ("flags", C.c_uint32)]
+
+
 class _PlanStep(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("commit", C.c_int32), ("directive", C.c_char_p), ("args", C.c_char_p),
                 ("from_stage", C.c_char_p), ("from_paths", C.POINTER(C.c_char_p)), ("n_paths", C.c_size_t)]
@@ -96,6 +100,8 @@ SYMBOLS = [
                                                               C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_describe_update_from_tar", C.c_size_t, [_P, C.c_int64, C.c_int, C.c_char_p, C.c_size_t, C.c_char_p,
                                                            C.c_size_t]),
+    ("mkhost_memfs_update_from_tars", C.c_int, [_P, _P, C.c_int64, C.POINTER(TarSpec), C.c_size_t, C.c_uint32,
+                                                C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
     ("mkhost_copy_op_execute", C.c_int, [C.POINTER(CopyOp), C.c_uint32, C.POINTER(C.c_char_p), C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_eval_symlinks", C.c_size_t, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_cache_key", C.c_size_t, [C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]),
@@ -378,6 +384,18 @@ class MemFS:
         if load().mkhost_memfs_update_from_tar(self.h, eng.h, now_unix, tar_fd, flags, C.byref(out), err, len(err)):
             raise HostError(err.value.decode())
         return _layer_dict(out)
+
+    def update_from_tars(self, eng: abi.Engine, now_unix: int, layers: Sequence, flags: int = 0):
+        """A run of layers applied in order in ONE engine session, their DiffID chains hashed together.  layers: tar_fd
+        or (tar_fd, per-layer flags such as MKHOST_GUNZIP) per layer.  -> one dict per layer, as update_from_tar gives;
+        root / n_chunks / n_unique are those of the whole run."""
+        n = len(layers)
+        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
+        for i, l in enumerate(layers):
+            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
+        if load().mkhost_memfs_update_from_tars(self.h, eng.h, now_unix, specs, n, flags, outs, err, len(err)):
+            raise HostError(err.value.decode())
+        return [_layer_dict(outs[i]) for i in range(n)]
 
     def commit_scan(self, eng: abi.Engine, now_unix: int, n_threads: int = 0, tar_fd: int = -1, flags: int = 0):
         err, out = C.create_string_buffer(1024), LayerResult()

@@ -363,41 +363,77 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
         m->fs.set_now(now_unix);
         const bool want_digest = !(flags & MKHOST_NO_TAR_DIGEST);
         ck(eng, mksnap_begin(eng), "begin");
-        const bool file_digests = (flags & MKHOST_FILE_DIGESTS) != 0;
-        ArenaTarSource src(eng, tar_fd, want_digest, file_digests);
-        GunzipSession gz;
-        if (flags & MKHOST_GUNZIP) {
-            const std::vector<uint8_t> blob = read_all(tar_fd);
-            gz.open(eng, blob);
-            src.gunzip = eng;
-        }
-        const bool untar = (flags & MKHOST_UNTAR) != 0;
-        src.allow_split = !untar; // untarOneItem writes a member from one contiguous body
-        MemFS::Untar u;
-        const std::vector<TarMember> members =
-            untar ? read_tar(src, [&](const TarMember &mem, const uint8_t *body) { m->fs.untar_member(u, mem, body); }) // files written from the arena
-                  : read_tar(src);
-        src.s.submit_tar(true);
+        IngestedLayer in;
+        ingest_layer(m->fs, eng, tar_fd, flags, 0, 0, 1, in);
         mksnap_result res;
-        const uint32_t n_files = src.s.n_file_streams;
-        const std::vector<uint8_t> d = src.s.finish(res, n_files + 1, want_digest || n_files);
-        const std::map<std::string, MemFile> layer = untar ? m->fs.untar_finish(u) : m->fs.update_from_tar(members);
-        set_layer_result(out, res, want_digest ? d.data() : nullptr, layer.size(), src.s.tar_bytes);
-        if (file_digests) { // remember the content digest of every regular member that made it into the tree
-            uint32_t k = 0;
-            for (const auto &mem : members) {
-                if (mem.hdr.typeflag != '0' || mem.data_len == 0)
-                    continue;
-                ++k;
-                const std::string dst = abs_path(mem.hdr.name);
-                auto it = layer.find(dst);
-                if (it != layer.end() && !it->second.whiteout && it->second.hdr.typeflag == '0')
-                    m->fs.set_digest(dst, d.data() + 32 * k);
-            }
-        }
+        ck(eng, mksnap_finish(eng, &res), "finish");
+        std::vector<uint8_t> d((in.n_file_streams + 1) * 32, 0);
+        if (want_digest || in.n_file_streams)
+            ck(eng, mksnap_get_stream_digests(eng, d.data(), in.n_file_streams + 1), "stream digests");
+        const std::map<std::string, MemFile> layer = merge_layer(m->fs, flags, in, d.data(), 1);
+        set_layer_result(out, res, want_digest ? d.data() : nullptr, layer.size(), in.tar_bytes);
         return 0;
     } catch (const std::exception &e) {
         set_err(err, errlen, std::string("update memfs from tar: ") + e.what());
+        return -1;
+    }
+}
+
+int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
+                                  size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
+{
+    try {
+        if (!m || !eng || (!layers && n_layers) || (!outs && n_layers))
+            throw HostError("null argument");
+        if (flags & ~(uint32_t)(MKHOST_NO_TAR_DIGEST | MKHOST_FILE_DIGESTS | MKHOST_UNTAR))
+            throw HostError("update from tars: flags take MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS and MKHOST_UNTAR; "
+                            "MKHOST_GUNZIP goes per layer");
+        for (size_t i = 0; i < n_layers; ++i)
+            if (layers[i].flags & ~(uint32_t)MKHOST_GUNZIP)
+                throw HostError("update from tars: layer " + std::to_string(i) + ": only MKHOST_GUNZIP is a per-layer flag");
+        if (n_layers == 0)
+            return 0;
+        m->fs.set_now(now_unix);
+        const bool want_digest = !(flags & MKHOST_NO_TAR_DIGEST);
+        const bool file_digests = (flags & MKHOST_FILE_DIGESTS) != 0;
+        const mksnap_limits lim = engine_limits(eng);
+        if (n_layers + (file_digests ? 1 : 0) > lim.max_streams)
+            throw HostError("a run of " + std::to_string(n_layers) + " layers needs a stream slot per layer" +
+                            (file_digests ? " and more for the per-file digests" : "") + ": engine max_extents (" +
+                            std::to_string(lim.max_streams) + ") is too small");
+        // layer i's DiffID is stream slot i, deferred: the engine keeps its bytes in the stream log and hashes the
+        // chains of the whole run together.  Per-file streams are inline, in the slots after the layers.
+        const uint32_t file_base = (uint32_t)n_layers;
+        ck(eng, mksnap_begin(eng), "begin");
+        if (want_digest)
+            ck(eng, mksnap_reserve_stream_log(eng, RUN_STREAM_LOG_BYTES), "reserve stream log");
+        std::vector<uint64_t> entries(n_layers), tar_bytes(n_layers);
+        std::vector<uint8_t> d;    // stream-digest rows [0, file_base + most file streams of a layer so far)
+        uint32_t max_files = 0;
+        for (size_t i = 0; i < n_layers; ++i) {
+            // the layers join the tree (and the disk) strictly in order: whiteouts, overwrites and hard links of
+            // layer i + 1 act on what layer i left
+            IngestedLayer in;
+            ingest_layer(m->fs, eng, layers[i].tar_fd, flags | layers[i].flags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in);
+            if (in.n_file_streams) { // inline streams: their rows are final once the submits so far have run
+                max_files = std::max(max_files, in.n_file_streams);
+                d.assign(((uint64_t)file_base + max_files) * 32, 0);
+                ck(eng, mksnap_get_stream_digests(eng, d.data(), file_base + max_files), "stream digests");
+            }
+            const std::map<std::string, MemFile> layer = merge_layer(m->fs, flags, in, d.data(), file_base);
+            entries[i] = layer.size();
+            tar_bytes[i] = in.tar_bytes;
+        }
+        mksnap_result res;
+        ck(eng, mksnap_finish(eng, &res), "finish");
+        std::vector<uint8_t> rows(std::max<uint64_t>(res.n_streams, n_layers) * 32, 0);
+        if (want_digest)
+            ck(eng, mksnap_get_stream_digests(eng, rows.data(), rows.size() / 32), "stream digests");
+        for (size_t i = 0; i < n_layers; ++i) // root: chunk table of the whole run (one session)
+            set_layer_result(&outs[i], res, want_digest ? rows.data() + 32 * i : nullptr, entries[i], tar_bytes[i]);
+        return 0;
+    } catch (const std::exception &e) {
+        set_err(err, errlen, std::string("update memfs from tars: ") + e.what());
         return -1;
     }
 }
