@@ -270,6 +270,37 @@ typedef struct {
 int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
                                   size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen);
 
+/* Block indexes of single-member gzip layers, remembered between builds.  A registry layer is one gzip member without
+ * flush points, which mksnap_gunzip_open decodes on one GPU thread; mksnap_gunzip_open_indexed records where its DEFLATE
+ * blocks start on the first decode, and later opens of the same blob take those points and decode in parallel.  The
+ * cache maps a caller key (makisu: the image store's file name, descriptor.Digest.Hex()) to the blob length and its
+ * points; an entry whose length differs from the blob's, or whose points are not ascending and inside the blob, is
+ * ignored.  A point the engine cannot link costs speed only, never output or an error, so a stale or foreign entry is
+ * harmless.  One cache per image store, owned by the caller; save/load keep it between processes (a file that does not
+ * parse fails the load and leaves the cache as it was).
+ * The _indexed calls equal mkhost_memfs_update_from_tar / _tars, except that each layer flagged MKHOST_GUNZIP that has a
+ * key (key, keys[i]; NULL = none) is opened by mksnap_gunzip_open_indexed with the cached points, and after the open
+ * succeeds its entry is replaced with what mksnap_gunzip_get_index returns.  With cache == NULL they are the plain
+ * calls.  stats (may be NULL) adds up over the call: blobs opened indexed, of them with a cached index, and the engine's
+ * points_given / points_linked / points_recorded. */
+typedef struct mkhost_gz_index_cache mkhost_gz_index_cache;
+typedef struct {
+    uint64_t blobs, blobs_with_index;
+    uint64_t points_given, points_linked, points_recorded;
+} mkhost_gz_index_stats;
+mkhost_gz_index_cache *mkhost_gz_index_cache_new(void);
+void mkhost_gz_index_cache_free(mkhost_gz_index_cache *c);
+uint64_t mkhost_gz_index_cache_size(const mkhost_gz_index_cache *c);
+int mkhost_gz_index_cache_save(const mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_gz_index_cache_load(mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_memfs_update_from_tar_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache, const char *key,
+                                         int64_t now_unix, int tar_fd, uint32_t flags, mkhost_layer_result *out,
+                                         mkhost_gz_index_stats *stats, char *err, size_t errlen);
+int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache,
+                                          const char *const *keys, int64_t now_unix, const mkhost_tar_spec *layers,
+                                          size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
+                                          mkhost_gz_index_stats *stats, char *err, size_t errlen);
+
 /* CopyOperation.Execute (lib/snapshot/copy_op.go:82-147) with fileio.Copier (lib/fileio/copy.go): what a COPY/ADD step
  * does to the file system when it runs with --modifyfs.  op->dst is used as the on-disk destination exactly like the
  * reference does (resolved against op->work_dir when relative).  mode selects the Copier of copy_op.go:98-124:

@@ -335,6 +335,33 @@ typedef struct {
     uint32_t extra_decodes;
 } mksnap_gunzip_times;
 int mksnap_gunzip_get_times(mksnap_t *h, mksnap_gunzip_times *out);
+/* Indexed open: for a single member without flush points (gzip CLI, compress/gzip, most registry layers), which the open
+ * above decodes on one GPU thread.  Like mksnap_gunzip_open, but positions are bit-granular: the candidate starts are
+ * the scanned ones (times 8) merged with `points`, bit offsets into the blob of DEFLATE block headers, strictly
+ * ascending and < 8 * gz_len (else MKSNAP_E_INVAL, and the handle stays usable); NULL / 0 = no index.  Every count
+ * decode records the first block header at least 1 MiB of output after its start or after its previous record, and
+ * each linked segment longer than 1 MiB is cut at the records of its decode, so the write decodes and the output window
+ * scale with 1 MiB pieces, not with the member.  A point is a candidate like any other: one that is not a block start
+ * (stale, another blob's, hostile) is never linked, so an index changes only the speed, never the output or an error.
+ * Reads, close and times as after mksnap_gunzip_open.
+ * Device memory on top of mksnap_gunzip_open's: 8 bytes per point in the candidate table and 32 per count result, a
+ * record buffer of 65536 records at 24 bytes (1.5 MiB), and 8 bytes per cut in the candidate table of the write
+ * decodes.  The records of all count decodes share that buffer, false candidates' decodes included, and records past it
+ * are dropped.  On a blob whose false candidates fill it first (adversarial input), the chain's own records can be
+ * lost: its segments stay long, and the output window is then max(256 MiB, largest segment) at 3 bytes per output
+ * byte, as for mksnap_gunzip_open.  The output is unchanged either way. */
+int mksnap_gunzip_open_indexed(mksnap_t *h, const void *gz, uint64_t gz_len, const uint64_t *points,
+                               uint64_t n_points, mksnap_gunzip_info *info);
+typedef struct {
+    uint64_t points_given;    /* n_points of the open */
+    uint64_t points_linked;   /* given points that start a linked segment */
+    uint64_t points_recorded; /* cuts taken from the records of this open */
+    uint64_t n_points;        /* points the index holds */
+} mksnap_gunzip_index_info;
+/* After an indexed open: the bit offsets worth remembering for the next open of the same blob, ascending (the starts of
+ * the linked segments that are not scanned candidates); min(cap, n_points) of them go to `points`.  MKSNAP_E_STATE
+ * when no gunzip is open or it was opened by mksnap_gunzip_open. */
+int mksnap_gunzip_get_index(mksnap_t *h, uint64_t *points, uint64_t cap, mksnap_gunzip_index_info *out);
 
 /* ---- result tables (valid after mksnap_finish, until the next begin) ---- */
 /* chunk END offsets (exclusive; position in the concatenation of all submitted

@@ -357,3 +357,94 @@ func (e *Engine) ContextCRC32Cached(cc *CrcCache, prefix []byte, contextDir stri
 	}
 	return uint32(c), uint64(st.bytes_sent), nil
 }
+
+// GzIndexCache remembers where the DEFLATE blocks of single-member gzip layers start, per image-store digest
+// (include/mkhost.h, "Block indexes of single-member gzip layers"): the first ingest of a base-image layer records the
+// index, later ingests of the same blob decode it in parallel on the GPU.  One cache per image store; Save/Load keep it
+// between makisu invocations.  A stale or foreign entry costs speed only, never output.
+type GzIndexCache struct{ c *C.mkhost_gz_index_cache }
+
+// NewGzIndexCache loads `path` when it exists ("" = start cold).
+func NewGzIndexCache(path string) (*GzIndexCache, error) {
+	gc := &GzIndexCache{c: C.mkhost_gz_index_cache_new()}
+	runtime.SetFinalizer(gc, func(gc *GzIndexCache) { C.mkhost_gz_index_cache_free(gc.c) })
+	if path == "" {
+		return gc, nil
+	}
+	if _, err := os.Stat(path); err != nil {
+		return gc, nil
+	}
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_gz_index_cache_load(gc.c, cpath, errBuf, errLen) != 0 {
+		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return gc, nil
+}
+
+// Save writes the cache (next to the image store).
+func (gc *GzIndexCache) Save(path string) error {
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_gz_index_cache_save(gc.c, cpath, errBuf, errLen) != 0 {
+		return fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return nil
+}
+
+// TarLayer is one layer of a run: the store file and its per-layer flags (Gunzip), and the key of its block index in
+// a GzIndexCache (descriptor.Digest.Hex(); "" = none).
+type TarLayer struct {
+	File  *os.File
+	Flags uint32
+	Key   string
+}
+
+// UpdateFromTarsIndexed applies a run of layers in order in one engine session (FromStep.Execute, buildNode.applyLayer),
+// each Gunzip layer with a key opened with the block index cached under it; gc == nil is the same run without an index.
+func (fs *MemFS) UpdateFromTarsIndexed(e *Engine, gc *GzIndexCache, now int64, layers []TarLayer, untar bool, flags uint32) ([]LayerResult, error) {
+	if untar {
+		flags |= 32 // MKHOST_UNTAR
+	}
+	n := len(layers)
+	if n == 0 {
+		return nil, nil
+	}
+	specs := make([]C.mkhost_tar_spec, n)
+	keys := make([]string, n)
+	for i, l := range layers {
+		specs[i].tar_fd = C.int(l.File.Fd())
+		specs[i].flags = C.uint32_t(l.Flags)
+		keys[i] = l.Key
+	}
+	ckeys, freeKeys := cStrings(keys)
+	defer freeKeys()
+	view := (*[1 << 28]*C.char)(unsafe.Pointer(ckeys))[:n:n]
+	for i := range keys {
+		if keys[i] == "" { // NULL key: this layer is opened without an index
+			C.free(unsafe.Pointer(view[i]))
+			view[i] = nil
+		}
+	}
+	var cache *C.mkhost_gz_index_cache
+	if gc != nil {
+		cache = gc.c
+	}
+	outs := make([]C.mkhost_layer_result, n)
+	var st C.mkhost_gz_index_stats
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	if rc := C.mkhost_memfs_update_from_tars_indexed(fs.m, e.h, cache, (**C.char)(unsafe.Pointer(ckeys)), C.int64_t(now),
+		&specs[0], C.size_t(n), C.uint32_t(flags), &outs[0], &st, errBuf, errLen); rc != 0 {
+		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	res := make([]LayerResult, n)
+	for i := range outs {
+		res[i] = toResult(&outs[i])
+	}
+	return res, nil
+}

@@ -97,6 +97,11 @@ class GunzipTimes(C.Structure):
                 ("ms_crc", C.c_float), ("extra_decodes", C.c_uint32)]
 
 
+class GunzipIndexInfo(C.Structure):
+    _fields_ = [("points_given", C.c_uint64), ("points_linked", C.c_uint64), ("points_recorded", C.c_uint64),
+                ("n_points", C.c_uint64)]
+
+
 # every symbol include/mksnap.h declares: (name, restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = [
@@ -129,6 +134,9 @@ SYMBOLS = [
     ("mksnap_gunzip_read", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("mksnap_gunzip_close", C.c_int, [_P]),
     ("mksnap_gunzip_get_times", C.c_int, [_P, C.POINTER(GunzipTimes)]),
+    ("mksnap_gunzip_open_indexed", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64), C.c_uint64,
+                                             C.POINTER(GunzipInfo)]),
+    ("mksnap_gunzip_get_index", C.c_int, [_P, C.POINTER(C.c_uint64), C.c_uint64, C.POINTER(GunzipIndexInfo)]),
     ("mksnap_get_chunks", C.c_int, [_P, _P, _P, C.c_uint64]),
     ("mksnap_get_table", C.c_int, [_P, _P, C.c_uint64]),
     ("mksnap_get_stream_digests", C.c_int, [_P, _P, C.c_uint64]),
@@ -307,6 +315,29 @@ class Engine:
         info = GunzipInfo()
         self._ck(self.lib.mksnap_gunzip_open(self.h, buf, len(b), C.byref(info)), "mksnap_gunzip_open")
         return info
+
+    def gunzip_open_indexed(self, blob, points=None) -> GunzipInfo:
+        """gunzip_open with a block index: `points` (ascending bit offsets of DEFLATE block headers, e.g. what
+        gunzip_index returned for the same blob) are extra segment starts; None records a new index."""
+        import numpy as np
+        b = memoryview(blob).cast("B")
+        buf = (C.c_uint8 * max(1, len(b))).from_buffer_copy(b) if len(b) else (C.c_uint8 * 1)()
+        pts = np.ascontiguousarray(points if points is not None else [], dtype=np.uint64)
+        info = GunzipInfo()
+        self._ck(self.lib.mksnap_gunzip_open_indexed(self.h, buf, len(b),
+                                                     pts.ctypes.data_as(C.POINTER(C.c_uint64)) if pts.size else None,
+                                                     pts.size, C.byref(info)), "mksnap_gunzip_open_indexed")
+        return info
+
+    def gunzip_index(self):
+        """(points, GunzipIndexInfo) of the gunzip opened by gunzip_open_indexed: the points to keep for the blob."""
+        import numpy as np
+        ix = GunzipIndexInfo()
+        self._ck(self.lib.mksnap_gunzip_get_index(self.h, None, 0, C.byref(ix)), "mksnap_gunzip_get_index")
+        pts = np.zeros(max(1, ix.n_points), dtype=np.uint64)
+        self._ck(self.lib.mksnap_gunzip_get_index(self.h, pts.ctypes.data_as(C.POINTER(C.c_uint64)), ix.n_points,
+                                                  C.byref(ix)), "mksnap_gunzip_get_index")
+        return pts[:ix.n_points], ix
 
     def gunzip_read(self, into) -> int:
         """Fill the writable buffer `into` with the next decompressed bytes; returns how many (short only at the end)."""

@@ -6,6 +6,7 @@
 //                                          00 00 FF FF, and every body start of the bitmap            (HBM, tiny)
 //   K5b k_gz_decode     count mode: speculative decode of every candidate, no output;                 (latency bound)
 //                       write mode: the true segments of one window, 16-bit symbols
+//       k_gz_decode_bits  the same for mksnap_gunzip_open_indexed: bit positions, count decodes record block starts
 //   K5c k_gz_resolve    window tails in segment order, one CTA                                        (latency, small)
 //   K5d k_gz_narrow     markers -> bytes, 16-bit symbols -> bytes                                     (HBM)
 //   K0  k_crc32_extents the CRC-32 of every member piece of the window (the context-CRC kernel as it is)
@@ -23,7 +24,9 @@
 // tables, two 32 KiB history buffers, and one output window of max(GZ_WINDOW, largest segment) bytes at 3 bytes per
 // output byte (16-bit symbols plus bytes), copied once per window to a pinned host buffer of the same size that the
 // reads copy from.  It does not grow with the decompressed length except through the largest segment: a member without
-// flush points is one segment.  Everything runs on the gunzip's own stream: reads interleaved with an ingest session
+// flush points is one segment, unless it is opened indexed: there segments are cut about every 1 MiB of output at
+// recorded block starts, and the open adds 8 bytes per point and per cut to the candidate tables, 32 per point to the
+// count results, and a record buffer of REC_CAP * 24 bytes (1.5 MiB).  Everything runs on the gunzip's own stream: reads interleaved with an ingest session
 // do not queue behind its kernels.
 #include "mksnap_inflate_core.h"
 
@@ -112,6 +115,29 @@ k_gz_decode(const uint8_t *__restrict__ gz, uint64_t gz_len, const uint64_t *__r
         atomicOr(bad, 1u);
 }
 
+// k_gz_decode of an indexed open: starts, candidates and segment ends are bit offsets, and count decodes record block
+// starts into `rec` (mksnap_inflate_core.h, Recorder).  A kernel of its own, so that k_gz_decode is unchanged.
+__global__ void __launch_bounds__(32 * DEC_WARPS)
+k_gz_decode_bits(const uint8_t *__restrict__ gz, uint64_t gz_len, const uint64_t *__restrict__ cand, uint64_t n_cand,
+                 const uint64_t *__restrict__ starts, uint64_t n, uint32_t K, mki::SegRes *__restrict__ res,
+                 const mki::Seg *__restrict__ segs, uint64_t win_off, uint16_t *__restrict__ sym,
+                 uint32_t *__restrict__ bad, mki::Recorder rec)
+{
+    const uint64_t i = (uint64_t)blockIdx.x * DEC_WARPS + (threadIdx.x >> 5);
+    if (i >= n || (threadIdx.x & 31u))
+        return;
+    mki::Tables t;
+    if (!segs) {
+        res[i] = mki::decode_segment_t<true>(gz, gz_len, starts[i], cand, n_cand, K, nullptr, 0, 0, &t, &rec);
+        return;
+    }
+    const mki::Seg s = segs[i];
+    const mki::SegRes r = mki::decode_segment_t<true>(gz, gz_len, s.start, cand, n_cand, mki::NO_LIMIT,
+                                                      sym + (s.out_off - win_off), s.out_len, s.member_pos, &t, nullptr);
+    if (r.status != (s.final ? mki::SEG_FINAL : mki::SEG_CAND) || r.end != s.end || r.out_len != s.out_len)
+        atomicOr(bad, 1u);
+}
+
 __global__ void __launch_bounds__(1024) k_gz_resolve(uint16_t *__restrict__ sym, const uint8_t *__restrict__ hist,
                                                      const mki::Seg *__restrict__ segs, uint64_t n, uint64_t win_off)
 {
@@ -186,6 +212,9 @@ struct mksnap_gunzip_state {
     uint64_t pos = 0;               // decompressed bytes handed out
     uint64_t fail_at = UINT64_MAX;  // the read that reaches this offset fails: a member with a bad trailer ends there
     bool broken = false;            // a window failed to decode: every later read fails
+    bool indexed = false;           // opened by mksnap_gunzip_open_indexed: bit positions, k_gz_decode_bits
+    std::vector<uint64_t> index;    // ... and the points mksnap_gunzip_get_index returns
+    mksnap_gunzip_index_info idx{};
     mksnap_gunzip_times times;
     cudaEvent_t ev[6];
 };
@@ -226,7 +255,8 @@ struct DevScratch {
 };
 
 // the body of mksnap_gunzip_open; on failure the caller frees the state
-int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_len, mksnap_gunzip_info *info)
+int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_len, const uint64_t *points,
+            uint64_t n_points, mksnap_gunzip_info *info)
 {
     // candidate counts and their scan are 32-bit: flush points alone are at most gz_len / 4 + 1; a blob whose member
     // headers push the total past that is refused after the count (MKSNAP_E_CAPACITY)
@@ -307,14 +337,42 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     CK(h, cudaGetLastError());
     CK(h, cudaFree(body.p)); // the bitmap is not needed past the scan: keep it out of the count pass's peak
     body.p = nullptr;
+
+    // indexed open: the candidates become bit offsets, merged with the caller's points
+    std::vector<uint64_t> byte_cand, bit_cand;
+    DevScratch rec, rec_n;
+    mki::Recorder recorder{nullptr, nullptr, mki::REC_CAP};
+    if (g->indexed) {
+        byte_cand.resize(g->n_cand);
+        CK(h, cudaMemcpyAsync(byte_cand.data(), g->d_cand, g->n_cand * 8, cudaMemcpyDeviceToHost, s));
+        CK(h, cudaStreamSynchronize(s));
+        bit_cand = mki::merge_points(byte_cand, points, n_points);
+        CK(h, cudaFree(g->d_cand));
+        g->d_cand = nullptr;
+        g->n_cand = bit_cand.size();
+        if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess)
+            return fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
+        CK(h, cudaMemcpyAsync(g->d_cand, bit_cand.data(), g->n_cand * 8, cudaMemcpyHostToDevice, s));
+        CK(h, cudaMalloc(&rec.p, mki::REC_CAP * sizeof(mki::Rec)));
+        CK(h, cudaMalloc(&rec_n.p, 8));
+        CK(h, cudaMemsetAsync(rec_n.p, 0, 8, s));
+        recorder.buf = (mki::Rec *)rec.p;
+        recorder.n = (unsigned long long *)rec_n.p;
+        st.pos *= 8;
+    }
     CK(h, cudaEventRecord(g->ev[1], s));
 
     // K5b count mode over every candidate
     CK(h, cudaMalloc(&g->d_res, g->n_cand * sizeof(mki::SegRes)));
     const uint64_t dgrid = (g->n_cand + gz::DEC_WARPS - 1) / gz::DEC_WARPS;
-    gz::k_gz_decode<<<(uint32_t)dgrid, 32 * gz::DEC_WARPS, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, g->d_cand,
-                                                                  g->n_cand, mki::K_PASS, g->d_res, nullptr, 0, nullptr,
-                                                                  nullptr);
+    if (g->indexed)
+        gz::k_gz_decode_bits<<<(uint32_t)dgrid, 32 * gz::DEC_WARPS, 0, s>>>(
+            g->d_gz, gz_len, g->d_cand, g->n_cand, g->d_cand, g->n_cand, mki::K_PASS, g->d_res, nullptr, 0, nullptr,
+            nullptr, recorder);
+    else
+        gz::k_gz_decode<<<(uint32_t)dgrid, 32 * gz::DEC_WARPS, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, g->d_cand,
+                                                                      g->n_cand, mki::K_PASS, g->d_res, nullptr, 0,
+                                                                      nullptr, nullptr);
     LAUNCH_OK(h);
     CK(h, cudaEventRecord(g->ev[2], s));
     std::vector<uint64_t> cand(g->n_cand);
@@ -342,8 +400,12 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
             mki::SegRes *const d_one_res = (mki::SegRes *)one_res.p;
             CK(h, cudaMemcpyAsync(d_one, &st.pos, 8, cudaMemcpyHostToDevice, s));
             CK(h, cudaEventRecord(g->ev[1], s));
-            gz::k_gz_decode<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT, d_one_res,
-                                             nullptr, 0, nullptr, nullptr);
+            if (g->indexed)
+                gz::k_gz_decode_bits<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
+                                                      d_one_res, nullptr, 0, nullptr, nullptr, recorder);
+            else
+                gz::k_gz_decode<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
+                                                 d_one_res, nullptr, 0, nullptr, nullptr);
             LAUNCH_OK(h);
             CK(h, cudaEventRecord(g->ev[2], s));
             CK(h, cudaMemcpyAsync(&r, d_one_res, sizeof r, cudaMemcpyDeviceToHost, s));
@@ -354,10 +416,11 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
         mki::Seg seg;
         mki::Member mem;
         bool ended = false;
-        const int lk = mki::link_feed(&st, r, gz, gz_len, &seg, &mem, &ended);
+        const int lk = g->indexed ? mki::link_feed<true>(&st, r, gz, gz_len, &seg, &mem, &ended)
+                                  : mki::link_feed(&st, r, gz, gz_len, &seg, &mem, &ended);
         if (lk == mki::LINK_ERR)
             return fail(h, MKSNAP_E_DATA, "gunzip: malformed data in member %u (compressed offset %llu)", st.member,
-                        (unsigned long long)st.pos);
+                        (unsigned long long)(g->indexed ? st.pos / 8 : st.pos));
         g->segs.push_back(seg);
         if (ended)
             g->mems.push_back(mem);
@@ -366,6 +429,26 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     }
     cudaFree(g->d_res);
     g->d_res = nullptr;
+    if (g->indexed) { // cut long segments at the records of their decode; the cuts join the write candidates
+        unsigned long long n_rec = 0;
+        CK(h, cudaMemcpyAsync(&n_rec, rec_n.p, 8, cudaMemcpyDeviceToHost, s));
+        CK(h, cudaStreamSynchronize(s));
+        std::vector<mki::Rec> recs(std::min<uint64_t>(n_rec, mki::REC_CAP));
+        CK(h, cudaMemcpyAsync(recs.data(), rec.p, recs.size() * sizeof(mki::Rec), cudaMemcpyDeviceToHost, s));
+        CK(h, cudaStreamSynchronize(s));
+        h->stats.d2h_bytes += recs.size() * sizeof(mki::Rec);
+        const mki::IndexCounts c = mki::split_segments(&g->segs, std::move(recs), &cand, byte_cand, points, n_points,
+                                                       &g->index);
+        g->idx = mksnap_gunzip_index_info{n_points, c.linked, c.recorded, g->index.size()};
+        if (c.recorded) {
+            CK(h, cudaFree(g->d_cand));
+            g->d_cand = nullptr;
+            g->n_cand = cand.size();
+            if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess)
+                return fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
+            CK(h, cudaMemcpyAsync(g->d_cand, cand.data(), g->n_cand * 8, cudaMemcpyHostToDevice, s));
+        }
+    }
 
     // windows of whole segments
     uint64_t max_seg = 0, max_mem_per_win = 1;
@@ -421,9 +504,15 @@ int gz_window_impl(mksnap *h, mksnap_gunzip_state *g)
     CK(h, cudaMemcpyAsync(g->d_seg_off, off.data(), n * 8, cudaMemcpyHostToDevice, s));
     CK(h, cudaMemsetAsync(g->d_bad, 0, 4, s));
     CK(h, cudaEventRecord(g->ev[0], s));
-    gz::k_gz_decode<<<(uint32_t)((n + gz::DEC_WARPS - 1) / gz::DEC_WARPS), 32 * gz::DEC_WARPS, 0, s>>>(
-        g->d_gz, g->gz_len, g->d_cand, g->n_cand, nullptr, n, mki::NO_LIMIT, nullptr, g->d_segs + w.seg0, w.out_off,
-        g->d_sym, g->d_bad);
+    const uint32_t dgrid = (uint32_t)((n + gz::DEC_WARPS - 1) / gz::DEC_WARPS);
+    if (g->indexed)
+        gz::k_gz_decode_bits<<<dgrid, 32 * gz::DEC_WARPS, 0, s>>>(g->d_gz, g->gz_len, g->d_cand, g->n_cand, nullptr, n,
+                                                                  mki::NO_LIMIT, nullptr, g->d_segs + w.seg0, w.out_off,
+                                                                  g->d_sym, g->d_bad, mki::Recorder{nullptr, nullptr, 0});
+    else
+        gz::k_gz_decode<<<dgrid, 32 * gz::DEC_WARPS, 0, s>>>(g->d_gz, g->gz_len, g->d_cand, g->n_cand, nullptr, n,
+                                                             mki::NO_LIMIT, nullptr, g->d_segs + w.seg0, w.out_off,
+                                                             g->d_sym, g->d_bad);
     LAUNCH_OK(h);
     CK(h, cudaEventRecord(g->ev[1], s));
     const uint8_t *hist = g->d_hist[g->hist_cur];
@@ -526,10 +615,11 @@ int gz_window(mksnap *h, mksnap_gunzip_state *g)
 
 } // namespace
 
-int mksnap_gunzip_open(mksnap_t *h, const void *gz, uint64_t gz_len, mksnap_gunzip_info *info)
+namespace {
+
+int gz_open_entry(mksnap_t *h, const void *gz, uint64_t gz_len, const uint64_t *points, uint64_t n_points, bool indexed,
+                  mksnap_gunzip_info *info)
 {
-    if (!h || (!gz && gz_len) || !info)
-        return MKSNAP_E_INVAL;
     if (h->gz)
         return fail(h, MKSNAP_E_STATE, "gunzip: already open (close it first)");
     CK(h, cudaSetDevice(h->cfg.device));
@@ -538,13 +628,48 @@ int mksnap_gunzip_open(mksnap_t *h, const void *gz, uint64_t gz_len, mksnap_gunz
     memset(&h->gz->times, 0, sizeof h->gz->times);
     for (cudaEvent_t &e : h->gz->ev)
         e = nullptr;
-    const int rc = gz_open(h, h->gz, (const uint8_t *)gz, gz_len, info);
+    h->gz->indexed = indexed;
+    const int rc = gz_open(h, h->gz, (const uint8_t *)gz, gz_len, points, n_points, info);
     if (rc) {
         gz_free(h);
         cudaGetLastError();
         memset(info, 0, sizeof *info);
     }
     return rc;
+}
+
+} // namespace
+
+int mksnap_gunzip_open(mksnap_t *h, const void *gz, uint64_t gz_len, mksnap_gunzip_info *info)
+{
+    if (!h || (!gz && gz_len) || !info)
+        return MKSNAP_E_INVAL;
+    return gz_open_entry(h, gz, gz_len, nullptr, 0, false, info);
+}
+
+int mksnap_gunzip_open_indexed(mksnap_t *h, const void *gz, uint64_t gz_len, const uint64_t *points,
+                               uint64_t n_points, mksnap_gunzip_info *info)
+{
+    if (!h || (!gz && gz_len) || !info || (!points && n_points))
+        return MKSNAP_E_INVAL;
+    for (uint64_t k = 0; k < n_points; ++k)
+        if (points[k] / 8 >= gz_len || (k && points[k] <= points[k - 1]))
+            return fail(h, MKSNAP_E_INVAL, "gunzip: index point %llu (bit %llu) is out of order or past the blob",
+                        (unsigned long long)k, (unsigned long long)points[k]);
+    return gz_open_entry(h, gz, gz_len, points, n_points, true, info);
+}
+
+int mksnap_gunzip_get_index(mksnap_t *h, uint64_t *points, uint64_t cap, mksnap_gunzip_index_info *out)
+{
+    if (!h || !out || (!points && cap))
+        return MKSNAP_E_INVAL;
+    if (!h->gz)
+        return fail(h, MKSNAP_E_STATE, "gunzip: not open");
+    if (!h->gz->indexed)
+        return fail(h, MKSNAP_E_STATE, "gunzip: not opened by mksnap_gunzip_open_indexed");
+    *out = h->gz->idx;
+    std::copy_n(h->gz->index.begin(), std::min<uint64_t>(cap, h->gz->index.size()), points);
+    return 0;
 }
 
 int mksnap_gunzip_read(mksnap_t *h, void *dst, uint64_t cap, uint64_t *got)

@@ -14,12 +14,22 @@
 // segment: in write mode those bytes become markers (0x8000 | index into that 32 KiB), which resolve_segment_tail()
 // and resolve_symbol() replace once the previous segments are known.
 //
+// Indexed open (mksnap_gunzip_open_indexed): the same decoder, link and candidate rule at bit granularity
+// (decode_segment_t<true>, link_feed<true>), so that a caller's points -- DEFLATE block headers at any bit -- are
+// candidates like the scanned ones.  Count decodes record a block start about every SPLIT_OUT output bytes (Recorder),
+// and split_segments() cuts each long linked segment at the records of its own decode: those are true block starts of
+// the chain with known output offsets, so a single member without flush points decodes in parallel after one serial
+// count pass, and the cuts are the index a later open of the same blob takes as points.
+//
 // Acceptance is zlib's raw inflate (stored / fixed / dynamic blocks, inftrees' rules on over-subscribed and incomplete
 // code sets, 286/287 and 30/31 invalid, a distance before the member start invalid) and Go's compress/gzip header and
 // multistream rules (FNAME / FCOMMENT at most 511 bytes, FHCRC checked, anything after a member that is not a member
 // header is an error, reserved flag bits ignored).
 #pragma once
 #include <stdint.h>
+
+#include <algorithm>
+#include <vector>
 
 #if defined(__CUDACC__)
 #define MKI_HD __host__ __device__
@@ -262,15 +272,48 @@ MKI_HD inline uint64_t upper_bound(const uint64_t *cand, uint64_t n, uint64_t x)
     return lo;
 }
 
+// ---- block-start records (mksnap_gunzip_open_indexed) ----------------------------------------------------------------
+// A count decode records the first block header at least SPLIT_OUT output bytes after its start or after its previous
+// record: its bit offset and its output offset in the segment.  Such a record is a true block start of that decode, so
+// a linked segment can be cut there without a second pass.  Records of all decodes share one bounded buffer; those past
+// its capacity are dropped, which only leaves a segment longer.
+constexpr uint64_t SPLIT_OUT = 1ull << 20;
+constexpr uint64_t REC_CAP = 1ull << 16; // records one open keeps (24 B each: 1.5 MiB)
+
+struct Rec {
+    uint64_t from; // start bit of the decode that recorded it
+    uint64_t bit;  // block header
+    uint64_t out;  // output bytes of that decode before the block
+};
+
+struct Recorder {
+    Rec *buf;
+    unsigned long long *n; // records offered (may exceed cap)
+    uint64_t cap;
+    MKI_HD void put(uint64_t from, uint64_t bit, uint64_t out) const
+    {
+#if defined(__CUDA_ARCH__)
+        const uint64_t k = atomicAdd(n, 1ull);
+#else
+        const uint64_t k = (*n)++;
+#endif
+        if (k < cap)
+            buf[k] = Rec{from, bit, out};
+    }
+};
+
 // Decode one segment from byte `start` of gz.
 //   count mode (out == nullptr): nothing is written; the decode stops (SEG_SUSPEND) once it has passed more than K
 //     candidates, so the speculative decodes of all candidates together read O(K * gz_len) bytes for any input.
 //   write mode: out[j] = byte j of the segment, or MARK | (32768 + j - dist) for a byte that copies from before the
 //     segment.  member_pos = output bytes of the member before the segment: a distance beyond that is an error.
 //     out_cap bounds what is written.
-MKI_HD inline SegRes decode_segment(const uint8_t *gz, uint64_t gz_len, uint64_t start, const uint64_t *cand,
-                                    uint64_t n_cand, uint32_t K, uint16_t *out, uint64_t out_cap, uint64_t member_pos,
-                                    Tables *t)
+//   BITS (mksnap_gunzip_open_indexed): `start`, the candidates and SegRes::end are bit offsets (SEG_FINAL: 8 times the
+//     trailer's byte offset), and a count-mode decode given `rec` records block starts (Recorder).
+template <bool BITS>
+MKI_HD inline SegRes decode_segment_t(const uint8_t *gz, uint64_t gz_len, uint64_t start, const uint64_t *cand,
+                                      uint64_t n_cand, uint32_t K, uint16_t *out, uint64_t out_cap, uint64_t member_pos,
+                                      Tables *t, const Recorder *rec)
 {
     static const uint16_t LBASE[29] = {3,  4,  5,  6,  7,  8,  9,  10, 11,  13,  15,  17,  19,  23, 27,
                                        31, 35, 43, 51, 59, 67, 83, 99, 115, 131, 163, 195, 227, 258};
@@ -279,14 +322,16 @@ MKI_HD inline SegRes decode_segment(const uint8_t *gz, uint64_t gz_len, uint64_t
                                        193, 257, 385, 513, 769, 1025, 1537, 2049, 3073, 4097, 6145, 8193, 12289, 16385, 24577};
     static const uint8_t DEXT[30] = {0, 0, 0, 0, 1, 1, 2, 2, 3, 3, 4, 4, 5, 5, 6, 6, 7, 7, 8, 8, 9, 9, 10, 10, 11, 11, 12, 12, 13, 13};
     SegRes r = {0, 0, 0, SEG_ERR, 0};
-    Bits b = {gz, gz_len, start, 0, 0};
+    const uint64_t start_byte = BITS ? start / 8 : start;
+    Bits b = {gz, gz_len, start_byte, 0, 0};
     uint64_t ci = upper_bound(cand, n_cand, start); // next candidate not yet passed
-    uint64_t next_bits = ci < n_cand ? cand[ci] * 8 : ~0ull;
+    uint64_t next_bits = ci < n_cand ? (BITS ? cand[ci] : cand[ci] * 8) : ~0ull;
     uint32_t passed = 0;
     uint64_t j = 0; // output position in the segment
+    uint64_t rec_at = SPLIT_OUT; // output position from which the next block start is recorded
 #define MKI_FAIL()                                  \
     do {                                            \
-        r.consumed = (b.bitpos() + 7) / 8 - start;  \
+        r.consumed = (b.bitpos() + 7) / 8 - start_byte; \
         r.out_len = j;                              \
         return r;                                   \
     } while (0)
@@ -295,14 +340,23 @@ MKI_HD inline SegRes decode_segment(const uint8_t *gz, uint64_t gz_len, uint64_t
     while ((p) > next_bits) {                                       \
         if (++passed > K) {                                         \
             r.status = SEG_SUSPEND;                                 \
-            r.consumed = cand[ci] + 1 - start;                      \
+            r.consumed = (BITS ? cand[ci] / 8 : cand[ci]) + 1 - start_byte; \
             r.out_len = j;                                          \
             return r;                                               \
         }                                                           \
         ++ci;                                                       \
-        next_bits = ci < n_cand ? cand[ci] * 8 : ~0ull;             \
+        next_bits = ci < n_cand ? (BITS ? cand[ci] : cand[ci] * 8) : ~0ull; \
+    }
+    if (BITS && (start & 7)) {
+        uint32_t v;
+        if (!b.get((uint32_t)(start & 7), &v))
+            MKI_FAIL();
     }
     for (;;) {
+        if (BITS && rec && j >= rec_at) {
+            rec->put(start, b.bitpos(), j);
+            rec_at = j + SPLIT_OUT;
+        }
         uint32_t final, type;
         if (!b.get(1, &final) || !b.get(2, &type))
             MKI_FAIL();
@@ -371,21 +425,28 @@ MKI_HD inline SegRes decode_segment(const uint8_t *gz, uint64_t gz_len, uint64_t
         const uint64_t bp = b.bitpos();
         if (final) {
             r.status = SEG_FINAL;
-            r.end = (bp + 7) / 8;
+            r.end = BITS ? (bp + 7) / 8 * 8 : (bp + 7) / 8;
             break;
         }
         MKI_PASS(bp);
         if (bp == next_bits) {
             r.status = SEG_CAND;
-            r.end = bp / 8;
+            r.end = BITS ? bp : bp / 8;
             break;
         }
     }
 #undef MKI_PASS
 #undef MKI_FAIL
     r.out_len = j;
-    r.consumed = r.end - start;
+    r.consumed = BITS ? (r.end - start) / 8 : r.end - start;
     return r;
+}
+
+MKI_HD inline SegRes decode_segment(const uint8_t *gz, uint64_t gz_len, uint64_t start, const uint64_t *cand,
+                                    uint64_t n_cand, uint32_t K, uint16_t *out, uint64_t out_cap, uint64_t member_pos,
+                                    Tables *t)
+{
+    return decode_segment_t<false>(gz, gz_len, start, cand, n_cand, K, out, out_cap, member_pos, t, nullptr);
 }
 
 // ---- gzip framing (RFC 1952, with Go compress/gzip's limits) -------------------------------------------------------
@@ -466,7 +527,7 @@ MKI_HD inline int64_t member_body(const uint8_t *gz, uint64_t gz_len, uint64_t q
 
 // ---- link: the true chain of segments through the speculative results --------------------------------------------
 struct Seg {
-    uint64_t start, end; // compressed byte range
+    uint64_t start, end; // compressed byte range (bit range after an indexed open)
     uint64_t out_off;    // offset in the decompressed stream
     uint64_t out_len;
     uint64_t member_pos; // output bytes of its member before it
@@ -480,7 +541,7 @@ struct Member {
 };
 
 struct LinkState {
-    uint64_t pos;       // start of the next segment
+    uint64_t pos;       // start of the next segment (a bit offset in BITS mode)
     uint64_t out;       // output bytes so far
     uint64_t mpos;      // output bytes of the current member so far
     uint32_t member;    // index of the current member
@@ -489,14 +550,16 @@ struct LinkState {
 
 enum : int { LINK_NEXT = 0, LINK_DONE = 1, LINK_ERR = -1 };
 
-// Start at the first member's header.  LINK_ERR: no valid member header at offset 0.
+// Start at the first member's header.  LINK_ERR: no valid member header at offset 0.  BITS: positions are bit offsets
+// (decode_segment_t<true>).
+template <bool BITS = false>
 MKI_HD inline int link_start(LinkState *st, const uint8_t *gz, uint64_t gz_len)
 {
     const int64_t body = parse_header(gz, gz_len, 0);
     *st = LinkState{0, 0, 0, 0, 0};
     if (body < 0)
         return LINK_ERR;
-    st->pos = (uint64_t)body;
+    st->pos = BITS ? (uint64_t)body * 8 : (uint64_t)body;
     return LINK_NEXT;
 }
 
@@ -504,6 +567,7 @@ MKI_HD inline int link_start(LinkState *st, const uint8_t *gz, uint64_t gz_len)
 // *seg, and *mem when the segment ends its member; returns LINK_NEXT (st->pos is the next start), LINK_DONE or
 // LINK_ERR.  After a final segment the trailer is read and whatever follows must be the end of the blob or another
 // member header.
+template <bool BITS = false>
 MKI_HD inline int link_feed(LinkState *st, const SegRes &r, const uint8_t *gz, uint64_t gz_len, Seg *seg, Member *mem,
                             bool *ended_member)
 {
@@ -517,7 +581,7 @@ MKI_HD inline int link_feed(LinkState *st, const SegRes &r, const uint8_t *gz, u
         st->pos = r.end;
         return LINK_NEXT;
     }
-    const uint64_t t = r.end;
+    const uint64_t t = BITS ? r.end / 8 : r.end;
     if (t + 8 > gz_len)
         return LINK_ERR;
     mem->out_off = st->out - st->mpos;
@@ -532,10 +596,74 @@ MKI_HD inline int link_feed(LinkState *st, const SegRes &r, const uint8_t *gz, u
     const int64_t body = parse_header(gz, gz_len, t + 8);
     if (body < 0)
         return LINK_ERR;
-    st->pos = (uint64_t)body;
+    st->pos = BITS ? (uint64_t)body * 8 : (uint64_t)body;
     st->mpos = 0;
     st->member++;
     return LINK_NEXT;
+}
+
+// ---- indexed open: the host steps around the count pass and the link --------------------------------------------------
+// Candidates of an indexed open: the scanned byte candidates as bit offsets, merged with the caller's points (bit
+// offsets, strictly ascending), without duplicates.
+inline std::vector<uint64_t> merge_points(const std::vector<uint64_t> &byte_cand, const uint64_t *points, uint64_t n)
+{
+    std::vector<uint64_t> out;
+    out.reserve(byte_cand.size() + n);
+    uint64_t i = 0, k = 0;
+    while (i < byte_cand.size() || k < n) {
+        const uint64_t v = k == n || (i < byte_cand.size() && byte_cand[i] * 8 <= points[k]) ? byte_cand[i++] * 8 : points[k++];
+        if (out.empty() || out.back() != v)
+            out.push_back(v);
+    }
+    return out;
+}
+
+struct IndexCounts {
+    uint64_t linked;   // given points that start a linked segment
+    uint64_t recorded; // cuts taken from records
+};
+
+// After the link: every segment that decodes to more than SPLIT_OUT bytes is cut at the records of the decode the link
+// followed (records with from == its start; a suspended count decode redone on the chain records the same blocks
+// twice).  `cand` (bit candidates) gains the cuts, so that the write decode of each piece ends exactly at the next one;
+// `index` gets the starts of the final segments that are not scanned candidates: the points worth giving a later open.
+inline IndexCounts split_segments(std::vector<Seg> *segs, std::vector<Rec> recs, std::vector<uint64_t> *cand,
+                                  const std::vector<uint64_t> &byte_cand, const uint64_t *points, uint64_t n_points,
+                                  std::vector<uint64_t> *index)
+{
+    IndexCounts c{0, 0};
+    std::sort(recs.begin(), recs.end(),
+              [](const Rec &a, const Rec &b) { return a.from != b.from ? a.from < b.from : a.bit < b.bit; });
+    std::vector<Seg> out;
+    std::vector<uint64_t> cuts;
+    for (const Seg &s : *segs) {
+        if (std::binary_search(points, points + n_points, s.start))
+            ++c.linked;
+        uint64_t bit = s.start, o = 0;
+        if (s.out_len > SPLIT_OUT) {
+            auto it = std::lower_bound(recs.begin(), recs.end(), s.start,
+                                       [](const Rec &r, uint64_t v) { return r.from < v; });
+            for (; it != recs.end() && it->from == s.start; ++it) {
+                if (it->bit <= bit || it->bit >= s.end || it->out <= o || it->out >= s.out_len)
+                    continue;
+                out.push_back(Seg{bit, it->bit, s.out_off + o, it->out - o, s.member_pos + o, s.member, 0});
+                cuts.push_back(it->bit);
+                bit = it->bit;
+                o = it->out;
+            }
+        }
+        out.push_back(Seg{bit, s.end, s.out_off + o, s.out_len - o, s.member_pos + o, s.member, s.final});
+    }
+    c.recorded = cuts.size();
+    std::vector<uint64_t> merged(cand->size() + cuts.size());
+    std::merge(cand->begin(), cand->end(), cuts.begin(), cuts.end(), merged.begin());
+    cand->swap(merged);
+    index->clear();
+    for (const Seg &s : out)
+        if (s.start % 8 || !std::binary_search(byte_cand.begin(), byte_cand.end(), s.start / 8))
+            index->push_back(s.start);
+    segs->swap(out);
+    return c;
 }
 
 // ---- resolve ------------------------------------------------------------------------------------------------------

@@ -35,6 +35,11 @@ class ChunkCacheStats(C.Structure):
                 ("bytes_chunked", C.c_uint64), ("bytes_uploaded", C.c_uint64)]
 
 
+class GzIndexStats(C.Structure):
+    _fields_ = [("blobs", C.c_uint64), ("blobs_with_index", C.c_uint64), ("points_given", C.c_uint64),
+                ("points_linked", C.c_uint64), ("points_recorded", C.c_uint64)]
+
+
 class LayerSpec(C.Structure):
     _fields_ = [("ops", C.POINTER(CopyOp)), ("n_ops", C.c_size_t), ("tar_fd", C.c_int)]
 
@@ -102,6 +107,18 @@ SYMBOLS = [
                                                            C.c_size_t]),
     ("mkhost_memfs_update_from_tars", C.c_int, [_P, _P, C.c_int64, C.POINTER(TarSpec), C.c_size_t, C.c_uint32,
                                                 C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
+    ("mkhost_gz_index_cache_new", _P, []),
+    ("mkhost_gz_index_cache_free", None, [_P]),
+    ("mkhost_gz_index_cache_size", C.c_uint64, [_P]),
+    ("mkhost_gz_index_cache_save", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_gz_index_cache_load", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_memfs_update_from_tar_indexed", C.c_int, [_P, _P, _P, C.c_char_p, C.c_int64, C.c_int, C.c_uint32,
+                                                       C.POINTER(LayerResult), C.POINTER(GzIndexStats), C.c_char_p,
+                                                       C.c_size_t]),
+    ("mkhost_memfs_update_from_tars_indexed", C.c_int, [_P, _P, _P, C.POINTER(C.c_char_p), C.c_int64,
+                                                        C.POINTER(TarSpec), C.c_size_t, C.c_uint32,
+                                                        C.POINTER(LayerResult), C.POINTER(GzIndexStats), C.c_char_p,
+                                                        C.c_size_t]),
     ("mkhost_copy_op_execute", C.c_int, [C.POINTER(CopyOp), C.c_uint32, C.POINTER(C.c_char_p), C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_eval_symlinks", C.c_size_t, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_cache_key", C.c_size_t, [C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]),
@@ -397,6 +414,31 @@ class MemFS:
             raise HostError(err.value.decode())
         return [_layer_dict(outs[i]) for i in range(n)]
 
+    def update_from_tar_indexed(self, eng: abi.Engine, cache: Optional["GzIndexCache"], key: Optional[str],
+                                now_unix: int, tar_fd: int, flags: int = 0):
+        """update_from_tar whose MKHOST_GUNZIP blob is opened with the block index cached under `key` (the image
+        store's digest hex), and leaves the index it returns there.  -> (result dict, stats dict)."""
+        err, out, st = C.create_string_buffer(1024), LayerResult(), GzIndexStats()
+        if load().mkhost_memfs_update_from_tar_indexed(self.h, eng.h, cache.h if cache is not None else None,
+                                                       key.encode() if key is not None else None, now_unix, tar_fd,
+                                                       flags, C.byref(out), C.byref(st), err, len(err)):
+            raise HostError(err.value.decode())
+        return _layer_dict(out), {k: getattr(st, k) for k, _ in GzIndexStats._fields_}
+
+    def update_from_tars_indexed(self, eng: abi.Engine, cache: Optional["GzIndexCache"], keys: Sequence,
+                                 now_unix: int, layers: Sequence, flags: int = 0):
+        """update_from_tars with a block-index cache: keys[i] (or None) for layer i.  -> (dicts, stats dict)."""
+        n = len(layers)
+        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
+        for i, l in enumerate(layers):
+            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
+        ks = (C.c_char_p * max(1, n))(*[k.encode() if k is not None else None for k in keys])
+        st = GzIndexStats()
+        if load().mkhost_memfs_update_from_tars_indexed(self.h, eng.h, cache.h if cache is not None else None, ks, now_unix, specs,
+                                                        n, flags, outs, C.byref(st), err, len(err)):
+            raise HostError(err.value.decode())
+        return [_layer_dict(outs[i]) for i in range(n)], {k: getattr(st, k) for k, _ in GzIndexStats._fields_}
+
     def commit_scan(self, eng: abi.Engine, now_unix: int, n_threads: int = 0, tar_fd: int = -1, flags: int = 0):
         err, out = C.create_string_buffer(1024), LayerResult()
         if load().mkhost_memfs_commit_scan(self.h, eng.h, now_unix, n_threads, tar_fd, flags, C.byref(out), err, len(err)):
@@ -517,6 +559,36 @@ class ChunkCache:
     def close(self):
         if getattr(self, "h", None):
             load().mkhost_chunk_cache_free(self.h)
+            self.h = None
+
+    __del__ = close
+
+
+class GzIndexCache:
+    """Block indexes of single-member gzip layers, per image-store digest, remembered between builds: a later ingest
+    of the same blob decodes it in parallel on the device (include/mkhost.h; MemFS.update_from_tar(s)_indexed)."""
+
+    def __init__(self, path: Optional[str] = None):
+        self.h = load().mkhost_gz_index_cache_new()
+        if path is not None and os.path.exists(path):
+            self.load(path)
+
+    def __len__(self):
+        return int(load().mkhost_gz_index_cache_size(self.h))
+
+    def load(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_gz_index_cache_load(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def save(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_gz_index_cache_save(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            load().mkhost_gz_index_cache_free(self.h)
             self.h = None
 
     __del__ = close

@@ -65,6 +65,11 @@ struct mkhost_crc_cache {
     std::map<std::string, Entry> files; // key: absolute path
 };
 
+// block indexes of gzip blobs per caller key, remembered between builds (include/mkhost.h)
+struct mkhost_gz_index_cache {
+    GzIndexMap map;
+};
+
 // chunk digests per source file, remembered between builds (incremental layer commit, include/mkhost.h)
 struct mkhost_chunk_cache {
     ChunkMemo memo;
@@ -356,15 +361,20 @@ size_t mkhost_memfs_describe_update_from_tar(mkhost_memfs *m, int64_t now_unix, 
     return mkhost_memfs_describe_update_from_tar_ex(m, now_unix, tar_fd, 0, out, cap, err, errlen);
 }
 
-int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
-                                 mkhost_layer_result *out, char *err, size_t errlen)
+} // extern "C"
+
+namespace {
+
+// mkhost_memfs_update_from_tar; with `ix`, mkhost_memfs_update_from_tar_indexed
+int update_from_tar_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
+                         mkhost_layer_result *out, const GzIndexUse *ix, char *err, size_t errlen)
 {
     try {
         m->fs.set_now(now_unix);
         const bool want_digest = !(flags & MKHOST_NO_TAR_DIGEST);
         ck(eng, mksnap_begin(eng), "begin");
         IngestedLayer in;
-        ingest_layer(m->fs, eng, tar_fd, flags, 0, 0, 1, in);
+        ingest_layer(m->fs, eng, tar_fd, flags, 0, 0, 1, in, ix);
         mksnap_result res;
         ck(eng, mksnap_finish(eng, &res), "finish");
         std::vector<uint8_t> d((in.n_file_streams + 1) * 32, 0);
@@ -379,8 +389,10 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
     }
 }
 
-int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
-                                  size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
+// mkhost_memfs_update_from_tars; with `cache`, mkhost_memfs_update_from_tars_indexed (keys[i] for layer i)
+int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
+                          size_t n_layers, uint32_t flags, mkhost_layer_result *outs, GzIndexMap *cache,
+                          const char *const *keys, mkhost_gz_index_stats *stats, char *err, size_t errlen)
 {
     try {
         if (!m || !eng || (!layers && n_layers) || (!outs && n_layers))
@@ -414,7 +426,9 @@ int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_un
             // the layers join the tree (and the disk) strictly in order: whiteouts, overwrites and hard links of
             // layer i + 1 act on what layer i left
             IngestedLayer in;
-            ingest_layer(m->fs, eng, layers[i].tar_fd, flags | layers[i].flags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in);
+            const GzIndexUse ix{cache, keys ? keys[i] : nullptr, stats};
+            ingest_layer(m->fs, eng, layers[i].tar_fd, flags | layers[i].flags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in,
+                         cache && ix.key ? &ix : nullptr);
             if (in.n_file_streams) { // inline streams: their rows are final once the submits so far have run
                 max_files = std::max(max_files, in.n_file_streams);
                 d.assign(((uint64_t)file_base + max_files) * 32, 0);
@@ -436,6 +450,102 @@ int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_un
         set_err(err, errlen, std::string("update memfs from tars: ") + e.what());
         return -1;
     }
+}
+
+} // namespace
+
+extern "C" {
+
+int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
+                                 mkhost_layer_result *out, char *err, size_t errlen)
+{
+    return update_from_tar_impl(m, eng, now_unix, tar_fd, flags, out, nullptr, err, errlen);
+}
+
+int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
+                                  size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
+{
+    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, nullptr, nullptr, nullptr, err, errlen);
+}
+
+int mkhost_memfs_update_from_tar_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache, const char *key,
+                                         int64_t now_unix, int tar_fd, uint32_t flags, mkhost_layer_result *out,
+                                         mkhost_gz_index_stats *stats, char *err, size_t errlen)
+{
+    const GzIndexUse ix{cache ? &cache->map : nullptr, key, stats};
+    return update_from_tar_impl(m, eng, now_unix, tar_fd, flags, out, cache && key ? &ix : nullptr, err, errlen);
+}
+
+int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache,
+                                          const char *const *keys, int64_t now_unix, const mkhost_tar_spec *layers,
+                                          size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
+                                          mkhost_gz_index_stats *stats, char *err, size_t errlen)
+{
+    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, cache ? &cache->map : nullptr,
+                                 keys, stats, err, errlen);
+}
+
+mkhost_gz_index_cache *mkhost_gz_index_cache_new(void) { return new mkhost_gz_index_cache; }
+void mkhost_gz_index_cache_free(mkhost_gz_index_cache *c) { delete c; }
+uint64_t mkhost_gz_index_cache_size(const mkhost_gz_index_cache *c) { return c ? c->map.e.size() : 0; }
+
+// "mkhost-gz-index-cache 1", then per blob a line "<gz_len> <n_points> <key>" followed by its points, 8 bytes each
+// (little endian)
+int mkhost_gz_index_cache_save(const mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen)
+{
+    FILE *f = c && path ? fopen(path, "wb") : nullptr;
+    if (!f) {
+        set_err(err, errlen, std::string("save gzip index cache: ") + strerror(errno));
+        return -1;
+    }
+    fprintf(f, "mkhost-gz-index-cache 1\n");
+    for (const auto &kv : c->map.e) { // keys with newlines are not cached
+        if (kv.first.find('\n') != std::string::npos)
+            continue;
+        fprintf(f, "%llu %zu %s\n", (unsigned long long)kv.second.gz_len, kv.second.points.size(), kv.first.c_str());
+        fwrite(kv.second.points.data(), 8, kv.second.points.size(), f);
+    }
+    const bool ok = !ferror(f) && fclose(f) == 0;
+    if (!ok)
+        set_err(err, errlen, std::string("save gzip index cache: ") + strerror(errno));
+    return ok ? 0 : -1;
+}
+
+int mkhost_gz_index_cache_load(mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen)
+{
+    FILE *f = c && path ? fopen(path, "rb") : nullptr;
+    if (!f) {
+        set_err(err, errlen, std::string("load gzip index cache: ") + strerror(errno));
+        return -1;
+    }
+    struct stat fst;
+    const uint64_t fsize = fstat(fileno(f), &fst) == 0 ? (uint64_t)fst.st_size : 0;
+    char *line = nullptr;
+    size_t cap = 0;
+    ssize_t n = getline(&line, &cap, f);
+    bool ok = n > 0 && strcmp(line, "mkhost-gz-index-cache 1\n") == 0;
+    std::map<std::string, GzIndexMap::Entry> e;
+    while (ok && (n = getline(&line, &cap, f)) > 0) {
+        if (line[n - 1] == '\n')
+            line[--n] = 0;
+        unsigned long long len = 0, pts = 0;
+        int used = 0;
+        if (sscanf(line, "%llu %llu %n", &len, &pts, &used) != 2 || used <= 0 || used >= n || pts > fsize / 8) {
+            ok = false; // the points must fit in what is left of the file
+            break;
+        }
+        GzIndexMap::Entry x{len, std::vector<uint64_t>(pts)};
+        ok = fread(x.points.data(), 8, pts, f) == pts;
+        e[line + used] = std::move(x);
+    }
+    free(line);
+    fclose(f);
+    if (!ok) {
+        set_err(err, errlen, "load gzip index cache: not a mkhost-gz-index-cache file");
+        return -1;
+    }
+    c->map.e.swap(e);
+    return 0;
 }
 
 // ---- cache.Manager wire format (lib/cache/cache_manager.go:34-35,239-252) ----
