@@ -386,47 +386,38 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
 
     // link: follow the true chain; starts without a usable count result are decoded again without the K limit
     DevScratch one, one_res; // the start and result of such a decode
-    for (;;) {
-        const uint64_t i = mki::upper_bound(cand.data(), g->n_cand, st.pos);
-        mki::SegRes r;
-        if (i > 0 && cand[i - 1] == st.pos && res[i - 1].status != mki::SEG_SUSPEND) {
-            r = res[i - 1];
-        } else {
-            if (!one.p) {
-                CK(h, cudaMalloc(&one.p, 8));
-                CK(h, cudaMalloc(&one_res.p, sizeof(mki::SegRes)));
-            }
-            uint64_t *const d_one = (uint64_t *)one.p;
-            mki::SegRes *const d_one_res = (mki::SegRes *)one_res.p;
-            CK(h, cudaMemcpyAsync(d_one, &st.pos, 8, cudaMemcpyHostToDevice, s));
-            CK(h, cudaEventRecord(g->ev[1], s));
-            if (g->indexed)
-                gz::k_gz_decode_bits<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
-                                                      d_one_res, nullptr, 0, nullptr, nullptr, recorder);
-            else
-                gz::k_gz_decode<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
-                                                 d_one_res, nullptr, 0, nullptr, nullptr);
-            LAUNCH_OK(h);
-            CK(h, cudaEventRecord(g->ev[2], s));
-            CK(h, cudaMemcpyAsync(&r, d_one_res, sizeof r, cudaMemcpyDeviceToHost, s));
-            CK(h, cudaStreamSynchronize(s));
-            g->times.ms_count += gz_ms(g, 1, 2);
-            g->times.extra_decodes++;
+    const auto redecode = [&](uint64_t pos, mki::SegRes *r) -> int {
+        if (!one.p) {
+            CK(h, cudaMalloc(&one.p, 8));
+            CK(h, cudaMalloc(&one_res.p, sizeof(mki::SegRes)));
         }
-        mki::Seg seg;
-        mki::Member mem;
-        bool ended = false;
-        const int lk = g->indexed ? mki::link_feed<true>(&st, r, gz, gz_len, &seg, &mem, &ended)
-                                  : mki::link_feed(&st, r, gz, gz_len, &seg, &mem, &ended);
-        if (lk == mki::LINK_ERR)
-            return fail(h, MKSNAP_E_DATA, "gunzip: malformed data in member %u (compressed offset %llu)", st.member,
-                        (unsigned long long)(g->indexed ? st.pos / 8 : st.pos));
-        g->segs.push_back(seg);
-        if (ended)
-            g->mems.push_back(mem);
-        if (lk == mki::LINK_DONE)
-            break;
-    }
+        uint64_t *const d_one = (uint64_t *)one.p;
+        mki::SegRes *const d_one_res = (mki::SegRes *)one_res.p;
+        CK(h, cudaMemcpyAsync(d_one, &pos, 8, cudaMemcpyHostToDevice, s));
+        CK(h, cudaEventRecord(g->ev[1], s));
+        if (g->indexed)
+            gz::k_gz_decode_bits<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
+                                                  d_one_res, nullptr, 0, nullptr, nullptr, recorder);
+        else
+            gz::k_gz_decode<<<1, 32, 0, s>>>(g->d_gz, gz_len, g->d_cand, g->n_cand, d_one, 1, mki::NO_LIMIT,
+                                             d_one_res, nullptr, 0, nullptr, nullptr);
+        LAUNCH_OK(h);
+        CK(h, cudaEventRecord(g->ev[2], s));
+        CK(h, cudaMemcpyAsync(r, d_one_res, sizeof *r, cudaMemcpyDeviceToHost, s));
+        CK(h, cudaStreamSynchronize(s));
+        g->times.ms_count += gz_ms(g, 1, 2);
+        g->times.extra_decodes++;
+        return 0;
+    };
+    const int lk = g->indexed ? mki::link_all<true>(&st, cand.data(), res.data(), g->n_cand, gz, gz_len, redecode,
+                                                    &g->segs, &g->mems)
+                              : mki::link_all<false>(&st, cand.data(), res.data(), g->n_cand, gz, gz_len, redecode,
+                                                     &g->segs, &g->mems);
+    if (lk == mki::LINK_ERR)
+        return fail(h, MKSNAP_E_DATA, "gunzip: malformed data in member %u (compressed offset %llu)", st.member,
+                    (unsigned long long)(g->indexed ? st.pos / 8 : st.pos));
+    if (lk != mki::LINK_DONE)
+        return lk;
     cudaFree(g->d_res);
     g->d_res = nullptr;
     if (g->indexed) { // cut long segments at the records of their decode; the cuts join the write candidates

@@ -1,8 +1,7 @@
 // mksnap_inflate_core.h -- the gzip / DEFLATE logic of the engine's gunzip (mksnap_gunzip_*), written once as
 // __host__ __device__ code: the kernels of mksnap_inflate.cuh run it on the H100, the engine's host side runs the link
-// step, and the CPU mock of the engine (tests/mock_engine/mock_mksnap_gunzip_members.cpp, the full candidate rule;
-// mock_mksnap_gunzip.cpp, flush points only) compiles the same file with g++, so the CPU tests fuzz the code that runs
-// on the GPU.
+// step, and the CPU mock of the engine (tests/mock_engine/mock_mksnap.cpp) compiles the same file with g++, so the CPU
+// tests fuzz the code that runs on the GPU.
 //
 // Segments.  A blob is cut at candidate starts (CAND_FLUSH, CAND_MEMBER below): the byte after every `00 00 FF FF` (the empty stored block
 // a sync or full flush ends with) and the body start of every byte-aligned member header the parser accepts, so that
@@ -600,6 +599,36 @@ MKI_HD inline int link_feed(LinkState *st, const SegRes &r, const uint8_t *gz, u
     st->mpos = 0;
     st->member++;
     return LINK_NEXT;
+}
+
+// The link over the count results (host only): from st->pos, take the result of the candidate that starts there, or
+// else call redecode(pos, &r) for a decode without the K limit (a start that is no candidate, or whose count decode
+// was suspended), and feed it to link_feed until the last member ends.  Returns LINK_DONE, LINK_ERR (st->member and
+// st->pos name the place), or the nonzero rc of redecode, which must differ from both.
+template <bool BITS, class Redecode>
+inline int link_all(LinkState *st, const uint64_t *cand, const SegRes *res, uint64_t n, const uint8_t *gz,
+                    uint64_t gz_len, Redecode &&redecode, std::vector<Seg> *segs, std::vector<Member> *mems)
+{
+    for (;;) {
+        const uint64_t i = upper_bound(cand, n, st->pos);
+        SegRes r;
+        if (i > 0 && cand[i - 1] == st->pos && res[i - 1].status != SEG_SUSPEND) {
+            r = res[i - 1];
+        } else if (const int rc = redecode(st->pos, &r)) {
+            return rc;
+        }
+        Seg seg;
+        Member mem;
+        bool ended = false;
+        const int lk = link_feed<BITS>(st, r, gz, gz_len, &seg, &mem, &ended);
+        if (lk == LINK_ERR)
+            return LINK_ERR;
+        segs->push_back(seg);
+        if (ended)
+            mems->push_back(mem);
+        if (lk == LINK_DONE)
+            return LINK_DONE;
+    }
 }
 
 // ---- indexed open: the host steps around the count pass and the link --------------------------------------------------

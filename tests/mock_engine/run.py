@@ -1,20 +1,15 @@
 """Entry point of a FRESH process (tests/test_host_mock_engine_cpu.py spawns it): load the CPU mock of the engine entry
 points with RTLD_GLOBAL first, so that libmkhost's mksnap_* references bind to it, then run one scenario.
     python -m tests.mock_engine.run <mock.so> <scenario> <tmpdir>"""
-import ctypes as C
 import sys
+
+from tests.mock_engine import load_for_child
 
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)          # BEFORE anything loads libmksnap / libmkhost
+    mock = load_for_child(mock_path, host=True)
     from tests.mock_engine import scenarios
-    from makisu_b200 import host
-    host.load()
-    # proof that the interposition worked: libmkhost's own view of mksnap_begin is the mock's
-    ours = C.cast(mock.mksnap_begin, C.c_void_p).value
-    seen = C.cast(C.CDLL(None).mksnap_begin, C.c_void_p).value
-    assert ours == seen, "libmkhost is not bound to the mock engine"
     getattr(scenarios, scenario)(scenarios.MockEngineFactory(mock), tmp)
     print("SCENARIO-OK", scenario)
 

@@ -1,19 +1,18 @@
 """CPU: incremental layer commit (mkhost_memfs_commit_copy_ops_cached) under the CPU mock of the engine
-(tests/mock_engine/mock_mksnap_chunks.cpp: mock_mksnap.cpp plus mksnap_chunks_add / mksnap_arena_submit_spans /
-mksnap_get_cdc / mksnap_get_chunks).  The mock zeroes every arena byte outside the spans of a sparse submit, as the
+(tests/mock_engine/mock_mksnap.cpp, with mksnap_chunks_add / mksnap_arena_submit_spans / mksnap_get_cdc /
+mksnap_get_chunks).  The mock zeroes every arena byte outside the spans of a sparse submit, as the
 device does, so a cached commit that leaves out a byte the engine reads gets a different root than the uncached one.
 Each scenario runs in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost:
     python -m tests.test_host_chunk_cache_cpu <mock.so> <scenario> <tmpdir>"""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import numpy as np
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
+from tests import mock_engine
+
 NOW = 1_600_000_000
 T = 1_500_000_000
 
@@ -87,22 +86,11 @@ def commit(eng, tmp, ctx, cache=None, flags=0, with_tar=True, tag="x"):
 
 
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    out = tmp_path_factory.mktemp("mock")
-    obj, so = str(out / "mkoracle.o"), str(out / "libmock_mksnap_chunks.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall",
-                           os.path.join(HERE, "mock_engine", "mock_mksnap_chunks.cpp"), obj, "-o", so])
-    return so
-
-
 @pytest.mark.parametrize("scenario", ["cold_warm_and_edited_no_tar_digest", "cold_warm_and_edited_tar_digest",
                                       "save_load_and_cdc_mismatch", "table_overflow_and_no_cache"])
-def test_cached_commit_against_the_mock_engine(mock_so, tmp_path, scenario):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_chunk_cache_cpu", mock_so, scenario, str(tmp_path)],
-                       cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "SCENARIO-OK" in r.stdout, r.stdout[-3000:] + r.stderr[-6000:]
+def test_cached_commit_against_the_mock_engine(tmp_path, scenario):
+    r = mock_engine.run("tests.test_host_chunk_cache_cpu", scenario, tmp_path)
+    assert "SCENARIO-OK" in r.stdout, r.stdout[-3000:]
 
 
 class _Engine:
@@ -288,11 +276,7 @@ def table_overflow_and_no_cache(mock, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
-    from makisu_b200 import host
-    host.load()
-    assert C.cast(mock.mksnap_chunks_add, C.c_void_p).value == C.cast(C.CDLL(None).mksnap_chunks_add, C.c_void_p).value, \
-        "libmkhost is not bound to the mock engine"
+    mock = mock_engine.load_for_child(mock_path, host=True)
     globals()[scenario](mock, tmp)
     print("SCENARIO-OK", scenario)
 

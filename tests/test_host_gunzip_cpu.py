@@ -1,8 +1,8 @@
 """CPU: gunzip (mksnap_gunzip_*) and update_from_tar(MKHOST_GUNZIP) under the CPU mock of the engine.
 
-The mock (tests/mock_engine/mock_mksnap_gunzip.cpp: mock_mksnap.cpp plus the gunzip entry points) runs the engine's own
-decoder, link and resolve code (makisu_b200/csrc/mksnap_inflate_core.h) step for step as the device does, so these
-tests check the code that runs on the GPU against Go's gzip reader (tests/gzip_corpus.py):
+The mock (tests/mock_engine/mock_mksnap.cpp) runs the engine's own candidate rule, decoder, link and resolve code
+(makisu_b200/csrc/mksnap_inflate_core.h) step for step as the device does, so these tests check the code that runs on
+the GPU against Go's gzip reader (tests/gzip_corpus.py):
   - the generated corpus, bit-exact, with Go's acceptance where Python's gzip differs;
   - a few thousand truncated or bit-flipped blobs through a mock built with ASan/UBSan: zlib's output or MKSNAP_E_DATA;
   - the work of the speculative decodes of a blob full of 00 00 FF FF stays linear in its size;
@@ -11,49 +11,20 @@ Each scenario runs in a fresh process that loads the mock with RTLD_GLOBAL befor
     python -m tests.test_host_gunzip_cpu <mock.so> <scenario> <tmpdir>"""
 import ctypes as C
 import os
-import subprocess
 import sys
 
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-
-def _build(out, sanitize):
-    obj, so = str(out / "mkoracle.o"), str(out / ("libmock_gunzip%s.so" % ("_asan" if sanitize else "")))
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    extra = ["-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer"] if sanitize else []
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", *extra,
-                           os.path.join(HERE, "mock_engine", "mock_mksnap_gunzip.cpp"), obj, "-o", so])
-    return so
-
-
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    return _build(tmp_path_factory.mktemp("mock"), False)
-
-
-def _run(so, scenario, tmp, env=None):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_gunzip_cpu", so, scenario, str(tmp)], cwd=ROOT,
-                       capture_output=True, text=True, env=env)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    return r
+from tests import mock_engine
 
 
 @pytest.mark.parametrize("scenario", ["corpus", "linear_work", "ingest"])
-def test_gunzip_mock(mock_so, tmp_path, scenario):
-    _run(mock_so, scenario, tmp_path)
+def test_gunzip_mock(tmp_path, scenario):
+    mock_engine.run("tests.test_host_gunzip_cpu", scenario, tmp_path)
 
 
-def test_fuzz_under_asan_ubsan(tmp_path_factory, tmp_path):
-    so = _build(tmp_path_factory.mktemp("mock_asan"), True)
-    env = dict(os.environ)
-    env["LD_PRELOAD"] = " ".join(subprocess.check_output(["gcc", "-print-file-name=" + l], text=True).strip()
-                                 for l in ("libasan.so", "libubsan.so"))
-    env["ASAN_OPTIONS"] = "detect_leaks=0"
-    r = _run(so, "fuzz", tmp_path, env)
-    assert "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-3000:]
+def test_fuzz_under_asan_ubsan(tmp_path):
+    r = mock_engine.run("tests.test_host_gunzip_cpu", "fuzz", tmp_path, sanitize=True)
     assert "fuzz ok" in r.stdout
 
 
@@ -175,14 +146,9 @@ def ingest(mock, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
+    mock = mock_engine.load_for_child(mock_path, host=scenario == "ingest")
     from tests import gzip_corpus as gc
     gc.bind(mock)
-    if scenario == "ingest":
-        from makisu_b200 import host
-        host.load()
-        assert C.cast(mock.mksnap_gunzip_open, C.c_void_p).value == \
-            C.cast(C.CDLL(None).mksnap_gunzip_open, C.c_void_p).value, "libmkhost is not bound to the mock engine"
     globals()[scenario](mock, tmp)
 
 

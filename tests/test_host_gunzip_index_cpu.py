@@ -2,8 +2,8 @@
 
 A single gzip member without flush points is one segment for mksnap_gunzip_open.  The indexed open records a block
 start about every 1 MiB of output while it decodes, cuts the member there, and returns the points, which a later open of
-the same blob takes as extra candidate starts.  The mock (tests/mock_engine/mock_mksnap_gunzip_index.cpp) runs the
-engine's decoder, link and cut (makisu_b200/csrc/mksnap_inflate_core.h); block starts come from libz
+the same blob takes as extra candidate starts.  The mock (tests/mock_engine/mock_mksnap.cpp) runs the engine's
+decoder, link and cut (makisu_b200/csrc/mksnap_inflate_core.h); block starts come from libz
 (tests/gzip_index.py), output from zlib with Go's gzip framing (tests/gzip_corpus.py):
   - corpus: levels 0-9, stored / fixed / dynamic blocks, single members of 4-64 MiB, multi-member, pgzip, BGZF and
     eStargz-shaped blobs: recorded points are libz block starts, a single member of at least 4 MiB gets several
@@ -19,50 +19,21 @@ engine's decoder, link and cut (makisu_b200/csrc/mksnap_inflate_core.h); block s
 Each scenario runs in a fresh process that loads the mock with RTLD_GLOBAL:
     python -m tests.test_host_gunzip_index_cpu <lib.so> <scenario> <tmpdir>"""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-
-def _build(out, sanitize):
-    obj, so = str(out / "mkoracle.o"), str(out / ("libmock_gunzip_index%s.so" % ("_asan" if sanitize else "")))
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    extra = ["-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer"] if sanitize else []
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", *extra,
-                           os.path.join(HERE, "mock_engine", "mock_mksnap_gunzip_index.cpp"), obj, "-o", so])
-    return so
-
-
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    return _build(tmp_path_factory.mktemp("mock"), False)
-
-
-def _run(so, scenario, tmp, env=None):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_gunzip_index_cpu", so, scenario, str(tmp)], cwd=ROOT,
-                       capture_output=True, text=True, env=env)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    return r
+from tests import mock_engine
+from tests.test_host_gunzip_cpu import _engine
 
 
 @pytest.mark.parametrize("scenario", ["corpus", "all_block_starts", "bad_indexes", "contract", "malformed", "ingest"])
-def test_index_mock(mock_so, tmp_path, scenario):
-    _run(mock_so, scenario, tmp_path)
+def test_index_mock(tmp_path, scenario):
+    mock_engine.run("tests.test_host_gunzip_index_cpu", scenario, tmp_path)
 
 
-def test_index_fuzz_under_asan_ubsan(tmp_path_factory, tmp_path):
-    so = _build(tmp_path_factory.mktemp("mock_asan"), True)
-    env = dict(os.environ)
-    env["LD_PRELOAD"] = " ".join(subprocess.check_output(["gcc", "-print-file-name=" + l], text=True).strip()
-                                 for l in ("libasan.so", "libubsan.so"))
-    env["ASAN_OPTIONS"] = "detect_leaks=0"
-    r = _run(so, "fuzz", tmp_path, env)
-    assert "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-3000:]
+def test_index_fuzz_under_asan_ubsan(tmp_path):
+    r = mock_engine.run("tests.test_host_gunzip_index_cpu", "fuzz", tmp_path, sanitize=True)
     assert "fuzz ok" in r.stdout
 
 
@@ -247,21 +218,16 @@ def fuzz(lib, h, n=3000):
 
 def ingest(mock, tmp):
     """Host: update_from_tar(s)_indexed through the cache on the mock engine (tests/gzip_index.py)."""
-    from makisu_b200 import host
     from tests import gzip_index as gi
     from tests.mock_engine.scenarios import MockEngineFactory
-    host.load()
-    assert C.cast(mock.mksnap_gunzip_open_indexed, C.c_void_p).value == \
-        C.cast(C.CDLL(None).mksnap_gunzip_open_indexed, C.c_void_p).value, "libmkhost is not bound to the mock engine"
     n = gi.check_ingest_indexed(MockEngineFactory(mock), tmp)
     print("ingest ok", n)
 
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
+    mock = mock_engine.load_for_child(mock_path, host=scenario == "ingest")
     from tests import gzip_index as gi
-    from tests.test_host_gunzip_cpu import _engine
     gi.bind(mock)
     if scenario == "ingest":
         ingest(mock, tmp)

@@ -2,7 +2,7 @@
 
 Every member body start is a candidate segment start, next to the flush points, so the members of such a blob are
 count-decoded in parallel and the link needs no decode of its own per member.  The mock
-(tests/mock_engine/mock_mksnap_gunzip_members.cpp) runs the engine's candidate rule, decoder and link
+(tests/mock_engine/mock_mksnap.cpp) runs the engine's candidate rule, decoder and link
 (makisu_b200/csrc/mksnap_inflate_core.h); expectations come from Go's reader restated over zlib (tests/gzip_corpus.py):
   - BGZF, eStargz, every header-flag combination, empty members, false candidates, members with flushes, headers across
     a scan-chunk edge, trailing garbage, zero padding, bad trailers and truncated headers (tests/gzip_members.py);
@@ -13,59 +13,25 @@ count-decoded in parallel and the link needs no decode of its own per member.  T
 Each scenario runs in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost:
     python -m tests.test_host_gunzip_members_cpu <mock.so> <scenario> <tmpdir>"""
 import ctypes as C
-import os
-import subprocess
 import sys
 
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-
-def _build(out, sanitize):
-    obj, so = str(out / "mkoracle.o"), str(out / ("libmock_gunzip_members%s.so" % ("_asan" if sanitize else "")))
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    extra = ["-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer"] if sanitize else []
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall", *extra,
-                           os.path.join(HERE, "mock_engine", "mock_mksnap_gunzip_members.cpp"), obj, "-o", so])
-    return so
-
-
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    return _build(tmp_path_factory.mktemp("mock"), False)
-
-
-def _run(so, scenario, tmp, env=None):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_gunzip_members_cpu", so, scenario, str(tmp)], cwd=ROOT,
-                       capture_output=True, text=True, env=env)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
-    return r
+from tests import mock_engine
+from tests.test_host_gunzip_cpu import _engine
 
 
 @pytest.mark.parametrize("scenario", ["cases", "candidates", "linear_work", "ingest"])
-def test_members_mock(mock_so, tmp_path, scenario):
-    _run(mock_so, scenario, tmp_path)
+def test_members_mock(tmp_path, scenario):
+    mock_engine.run("tests.test_host_gunzip_members_cpu", scenario, tmp_path)
 
 
-def test_members_fuzz_under_asan_ubsan(tmp_path_factory, tmp_path):
-    so = _build(tmp_path_factory.mktemp("mock_asan"), True)
-    env = dict(os.environ)
-    env["LD_PRELOAD"] = " ".join(subprocess.check_output(["gcc", "-print-file-name=" + l], text=True).strip()
-                                 for l in ("libasan.so", "libubsan.so"))
-    env["ASAN_OPTIONS"] = "detect_leaks=0"
-    r = _run(so, "fuzz", tmp_path, env)
-    assert "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-3000:]
+def test_members_fuzz_under_asan_ubsan(tmp_path):
+    r = mock_engine.run("tests.test_host_gunzip_members_cpu", "fuzz", tmp_path, sanitize=True)
     assert "fuzz ok" in r.stdout
 
 
 # ---------------------------------------------------------------------------------------------------------------
-def _engine(mock):
-    from tests.test_host_gunzip_cpu import _engine as eng
-    return eng(mock)
-
-
 def _candidates(mock):
     mock.mock_gunzip_candidate.restype = C.c_uint32
     mock.mock_gunzip_candidate.argtypes = [C.c_uint64, C.POINTER(C.c_uint64)]
@@ -200,14 +166,9 @@ def ingest(mock, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
+    mock = mock_engine.load_for_child(mock_path, host=scenario == "ingest")
     from tests import gzip_corpus as gc
     gc.bind(mock)
-    if scenario == "ingest":
-        from makisu_b200 import host
-        host.load()
-        assert C.cast(mock.mksnap_gunzip_open, C.c_void_p).value == \
-            C.cast(C.CDLL(None).mksnap_gunzip_open, C.c_void_p).value, "libmkhost is not bound to the mock engine"
     globals()[scenario](mock, tmp)
 
 

@@ -1,26 +1,13 @@
-"""CPU: libmkhost's engine-facing packers run against a CPU mock of the seven libmksnap entry points they call
-(tests/mock_engine/mock_mksnap.cpp: every digest computed by the oracle, the same call contract enforced).  Each
-scenario runs in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost, so the real host code -- arena
-flushing, stream continuation, ranges per file, untar / materialise from the arena -- executes exactly as it does on
-an H100, minus the kernels.  These are the CPU twins of tests/test_gpu_host.py and tests/test_gpu_host_arena_paths.py."""
+"""CPU: libmkhost's engine-facing packers run against the CPU mock of libmksnap (tests/mock_engine/mock_mksnap.cpp:
+every digest computed by the oracle, the same call contract enforced).  Each scenario runs in a fresh process that
+loads the mock with RTLD_GLOBAL before libmkhost, so the real host code -- arena flushing, stream continuation, ranges
+per file, untar / materialise from the arena -- executes exactly as it does on an H100, minus the kernels.  These are
+the CPU twins of tests/test_gpu_host.py and tests/test_gpu_host_arena_paths.py."""
 import os
-import subprocess
-import sys
 
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    out = tmp_path_factory.mktemp("mock")
-    obj, so = str(out / "mkoracle.o"), str(out / "libmock_mksnap.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall",
-                           os.path.join(HERE, "mock_engine", "mock_mksnap.cpp"), obj, "-o", so])
-    return so
+from tests import mock_engine
 
 
 @pytest.mark.skipif(os.geteuid() != 0, reason="chown needs root")
@@ -28,8 +15,6 @@ def mock_so(tmp_path_factory):
                                       "materialize_from_the_arena", "random_trees_small_arenas",
                                       "table_limits_and_arena_leases", "batch_of_layers_in_one_session",
                                       "ingest_member_larger_than_the_arena", "incremental_cache_id"])
-def test_host_packers_against_the_mock_engine(mock_so, tmp_path, scenario):
-    r = subprocess.run([sys.executable, "-m", "tests.mock_engine.run", mock_so, scenario, str(tmp_path)], cwd=ROOT,
-                       capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "SCENARIO-OK" in r.stdout, r.stdout[-3000:] + r.stderr[-6000:]
-    assert "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-6000:]  # tests/run_host_sanitized.sh
+def test_host_packers_against_the_mock_engine(tmp_path, scenario):
+    r = mock_engine.run("tests.mock_engine.run", scenario, tmp_path)
+    assert "SCENARIO-OK" in r.stdout, r.stdout[-3000:]

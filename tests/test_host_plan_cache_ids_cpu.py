@@ -2,12 +2,10 @@
 
 The oracle chain (tests/plan_oracle.py) is checked against hand-chained per-step oracle calls, mksnap_crc_prepend
 against zlib, and the host plan logic of libmkhost against the oracle under the CPU mock of the engine
-(tests/mock_engine/mock_mksnap_plan.cpp: mock_mksnap.cpp plus the fold entry points, k_crc_fold restated with the
-oracle's arithmetic).  Mock scenarios run in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost:
+(tests/mock_engine/mock_mksnap.cpp, whose fold entry points restate k_crc_fold with the oracle's arithmetic).  Mock
+scenarios run in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost:
     python -m tests.test_host_plan_cache_ids_cpu <mock.so> <scenario> <tmpdir>"""
-import ctypes as C
 import os
-import subprocess
 import sys
 import zlib
 
@@ -17,10 +15,8 @@ import pytest
 from makisu_b200 import abi
 from makisu_b200.host import PlanStep
 from oracle import ctx_crc
-from tests import plan_oracle
+from tests import mock_engine, plan_oracle
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 T = 1_500_000_000
 
 
@@ -128,23 +124,11 @@ def test_crc_prepend_matches_zlib():
 # ---------------------------------------------------------------------------------------------------------------
 # host plan logic under the mock engine
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    out = tmp_path_factory.mktemp("mock")
-    obj, so = str(out / "mkoracle.o"), str(out / "libmock_mksnap_plan.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-Wall",
-                           os.path.join(HERE, "mock_engine", "mock_mksnap_plan.cpp"), obj, "-o", so])
-    return so
-
-
 @pytest.mark.parametrize("scenario", ["ids_and_bytes_sent", "warm_cache_and_one_touched_file", "more_steps_than_stream_slots",
                                       "extent_table_overrun_is_an_error"])
-def test_plan_against_the_mock_engine(mock_so, tmp_path, scenario):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_plan_cache_ids_cpu", mock_so, scenario, str(tmp_path)],
-                       cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "SCENARIO-OK" in r.stdout, r.stdout[-3000:] + r.stderr[-6000:]
-    assert "runtime error" not in r.stderr and "AddressSanitizer" not in r.stderr, r.stderr[-6000:]
+def test_plan_against_the_mock_engine(tmp_path, scenario):
+    r = mock_engine.run("tests.test_host_plan_cache_ids_cpu", scenario, tmp_path)
+    assert "SCENARIO-OK" in r.stdout, r.stdout[-3000:]
 
 
 def _engine(factory, arena=1 << 20, max_extents=1 << 10):
@@ -244,12 +228,8 @@ def extent_table_overrun_is_an_error(factory, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
-    from makisu_b200 import host
+    mock = mock_engine.load_for_child(mock_path, host=True)
     from tests.mock_engine.scenarios import MockEngineFactory
-    host.load()
-    assert C.cast(mock.mksnap_crc_fold, C.c_void_p).value == C.cast(C.CDLL(None).mksnap_crc_fold, C.c_void_p).value, \
-        "libmkhost is not bound to the mock engine"
     globals()[scenario](MockEngineFactory(mock), tmp)
     print("SCENARIO-OK", scenario)
 

@@ -1,33 +1,22 @@
 """CPU: mkhost_memfs_update_from_tars (a run of layers in one engine session, DiffID chains deferred to the stream log)
-under the CPU mock engine (tests/mock_engine/mock_mksnap_defer.cpp).  In each case the run equals one
+under the CPU mock engine (tests/mock_engine/mock_mksnap.cpp).  In each case the run equals one
 update_from_tar call per layer (tests/apply_layers.py): per-layer DiffID, entries and tar bytes, the tree (a probe layer
 described against it), remembered file digests and, under MKHOST_UNTAR, the files on disk.  Layers: whiteouts and
 overwrites of what an earlier layer added, a hard link to an earlier layer's file, an empty layer, gzip and plain blobs,
 a member larger than the arena (without untar); a damaged layer in the middle leaves the layers before it merged.
 Each scenario runs in a fresh process that loads the mock with RTLD_GLOBAL before libmkhost:
     python -m tests.test_host_update_from_tars_cpu <mock.so> <scenario> <tmpdir>"""
-import ctypes as C
 import os
-import subprocess
 import sys
 
 import pytest
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-
-
-@pytest.fixture(scope="module")
-def mock_so(tmp_path_factory):
-    from tests.test_stream_defer_cpu import build_mock
-    return build_mock(tmp_path_factory.mktemp("mock_tars"))
+from tests import mock_engine
 
 
 @pytest.mark.parametrize("scenario", ["run", "damaged_layer", "too_few_slots", "no_layers"])
-def test_update_from_tars_mock(mock_so, tmp_path, scenario):
-    r = subprocess.run([sys.executable, "-m", "tests.test_host_update_from_tars_cpu", mock_so, scenario, str(tmp_path)],
-                       cwd=ROOT, capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout[-3000:] + r.stderr[-3000:]
+def test_update_from_tars_mock(tmp_path, scenario):
+    r = mock_engine.run("tests.test_host_update_from_tars_cpu", scenario, tmp_path)
     assert "SCENARIO-OK" in r.stdout
 
 
@@ -140,12 +129,8 @@ def no_layers(make, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    mock = C.CDLL(mock_path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
-    from makisu_b200 import host
+    mock = mock_engine.load_for_child(mock_path, host=True)
     from tests.mock_engine.scenarios import MockEngineFactory
-    host.load()
-    assert C.cast(mock.mksnap_reserve_stream_log, C.c_void_p).value == \
-        C.cast(C.CDLL(None).mksnap_reserve_stream_log, C.c_void_p).value, "libmkhost is not bound to the mock engine"
     globals()[scenario](MockEngineFactory(mock), tmp)
     print("SCENARIO-OK", scenario)
 

@@ -2,17 +2,14 @@
 (tests/mock_engine/mock_mksnap.cpp) runs continued_mix, long_streams and the contract table, so that the mock and the
 device engine (tests/test_gpu_stream_sha.py) are held to one table."""
 import ctypes as C
+import functools
 import hashlib
-import os
-import subprocess
 
 import numpy as np
 import pytest
 
+from tests import mock_engine
 from tests import stream_cases as sc
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -166,22 +163,17 @@ def test_generators_are_deterministic(name):
 # ---------------------------------------------------------------------------------------------------------------
 # the CPU mock engine on the same cases
 # ---------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def mock_lib(tmp_path_factory):
-    out = tmp_path_factory.mktemp("mock_streams")
-    obj, so = str(out / "mkoracle.o"), str(out / "libmock_mksnap.so")
-    subprocess.check_call(["gcc", "-O2", "-fPIC", "-c", os.path.join(ROOT, "oracle", "mkoracle.c"), "-o", obj])
-    # -Bsymbolic: the mock's own calls bind inside it even when libmksnap or the oracle is loaded globally
-    subprocess.check_call(["g++", "-O2", "-std=c++17", "-fPIC", "-shared", "-Wall", "-Wl,-Bsymbolic",
-                           os.path.join(HERE, "mock_engine", "mock_mksnap.cpp"), obj, "-o", so])
-    lib = C.CDLL(so)
+@functools.cache
+def _lib():
+    """The mock loaded into this process (RTLD_LOCAL: nothing else binds to it)."""
+    lib = C.CDLL(mock_engine.build())
     P, U64 = C.c_void_p, C.c_uint64
     for name, res, args in (("mksnap_create", C.c_int, [P, C.POINTER(P)]), ("mksnap_destroy", None, [P]),
                             ("mksnap_last_error", C.c_char_p, [P]), ("mksnap_begin", C.c_int, [P]),
                             ("mksnap_arena_acquire", C.c_int, [P, C.POINTER(P), C.POINTER(U64), C.POINTER(C.c_int32)]),
                             ("mksnap_arena_submit", C.c_int, [P, C.c_int32, U64, P, U64, P, U64]),
-                            ("mksnap_finish", C.c_int, [P, P]),
-                            ("mksnap_get_stream_digests", C.c_int, [P, P, U64])):
+                            ("mksnap_finish", C.c_int, [P, P]), ("mksnap_reserve_stream_log", C.c_int, [P, U64]),
+                            ("mksnap_get_stream_digests", C.c_int, [P, P, U64]), ("mock_log_flushes", U64, [P])):
         fn = getattr(lib, name)
         fn.restype, fn.argtypes = res, args
     return lib
@@ -190,12 +182,12 @@ def mock_lib(tmp_path_factory):
 class MockDriver:
     """stream_cases' driver interface over the CPU mock: pinned-arena style submits (acquire, copy, submit)."""
 
-    def __init__(self, lib, arena_bytes: int, max_extents: int):
+    def __init__(self, arena_bytes: int, max_extents: int):
         from makisu_b200.abi import Config
-        self.lib, self.h = lib, C.c_void_p()
+        self.lib, self.h = _lib(), C.c_void_p()
         cfg = Config()
         cfg.n_host_arenas, cfg.host_arena_bytes, cfg.max_extents = 2, arena_bytes, max_extents
-        assert lib.mksnap_create(C.byref(cfg), C.byref(self.h)) == 0
+        assert self.lib.mksnap_create(C.byref(cfg), C.byref(self.h)) == 0
 
     def close(self):
         self.lib.mksnap_destroy(self.h)
@@ -230,9 +222,9 @@ class MockDriver:
 
 
 @pytest.mark.parametrize("name", sc.MULTI_SUBMIT)
-def test_mock_engine_runs_the_stream_cases(mock_lib, name):
+def test_mock_engine_runs_the_stream_cases(name):
     c = sc.case(name)
-    d = MockDriver(mock_lib, c.arena_bytes, c.max_extents)
+    d = MockDriver(c.arena_bytes, c.max_extents)
     try:
         sc.run_case(d, c)
     finally:
@@ -240,8 +232,8 @@ def test_mock_engine_runs_the_stream_cases(mock_lib, name):
 
 
 @pytest.mark.parametrize("outcome", sc.contract(), ids=lambda o: o.name)
-def test_mock_engine_keeps_the_stream_contract(mock_lib, outcome):
-    d = MockDriver(mock_lib, sc.CONTRACT_ARENA, sc.CONTRACT_MAX)
+def test_mock_engine_keeps_the_stream_contract(outcome):
+    d = MockDriver(sc.CONTRACT_ARENA, sc.CONTRACT_MAX)
     try:
         sc.run_outcome(d, outcome)
     finally:
