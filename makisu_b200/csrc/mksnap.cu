@@ -16,6 +16,7 @@
 #include <algorithm>
 #include <string>
 #include <unordered_map>
+#include <utility>
 #include <vector>
 
 using namespace mk;
@@ -26,6 +27,90 @@ struct Id128 {
 
 namespace {
 
+// Owner of n elements of T, in device memory (cudaMalloc) or pinned host memory (cudaHostAlloc).  alloc() frees the
+// old block before it allocates, so a growth never holds both, and records n only when the allocation succeeds: after
+// a failed growth size() is 0, and a capacity check against it grows again or refuses rather than use a null pointer.
+template <typename T, bool Pinned> class Buf {
+public:
+    Buf() = default;
+    Buf(Buf &&o) noexcept : p_(std::exchange(o.p_, nullptr)), n_(std::exchange(o.n_, 0)) {}
+    Buf &operator=(Buf &&o) noexcept
+    {
+        std::swap(p_, o.p_);
+        std::swap(n_, o.n_);
+        return *this;
+    }
+    ~Buf() { reset(); }
+
+    cudaError_t alloc(uint64_t n)
+    {
+        reset();
+        void *q = nullptr;
+        cudaError_t e;
+        if constexpr (Pinned)
+            e = cudaHostAlloc(&q, n * sizeof(T), cudaHostAllocDefault);
+        else
+            e = cudaMalloc(&q, n * sizeof(T));
+        if (e == cudaSuccess) {
+            p_ = static_cast<T *>(q);
+            n_ = n;
+        }
+        return e;
+    }
+    void reset()
+    {
+        if (!p_)
+            return;
+        if constexpr (Pinned)
+            cudaFreeHost(p_);
+        else
+            cudaFree(p_);
+        p_ = nullptr;
+        n_ = 0;
+    }
+    uint64_t size() const { return n_; }
+    T *get() const { return p_; }
+    operator T *() const { return p_; }
+    T *operator->() const { return p_; }
+
+private:
+    T *p_ = nullptr;
+    uint64_t n_ = 0;
+};
+template <typename T> using DevBuf = Buf<T, false>;
+template <typename T> using PinnedBuf = Buf<T, true>;
+
+// Owner of one CUDA event or stream.  put() destroys what it holds and returns the slot a create call writes.
+template <typename H, cudaError_t (*Destroy)(H)> class Handle {
+public:
+    Handle() = default;
+    Handle(Handle &&o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+    Handle &operator=(Handle &&o) noexcept
+    {
+        std::swap(h_, o.h_);
+        return *this;
+    }
+    ~Handle()
+    {
+        if (h_)
+            Destroy(h_);
+    }
+
+    H *put()
+    {
+        if (h_)
+            Destroy(h_);
+        h_ = nullptr;
+        return &h_;
+    }
+    operator H() const { return h_; }
+
+private:
+    H h_ = nullptr;
+};
+using Event = Handle<cudaEvent_t, cudaEventDestroy>;
+using Stream = Handle<cudaStream_t, cudaStreamDestroy>;
+
 thread_local std::string g_create_error;
 
 constexpr uint64_t SLOT_SLACK = 8192;
@@ -35,25 +120,25 @@ constexpr int GH_WORDS = 8; // u64 words per rank in the all-gather header
 
 struct MetaSet {
     // pinned host staging
-    CrcExtent *h_crc = nullptr;
-    uint32_t *h_piece_base = nullptr;
-    CdcFile *h_files = nullptr;
-    uint64_t *h_rstart = nullptr, *h_rlen = nullptr;
-    uint32_t *h_rstream = nullptr, *h_rflags = nullptr;
+    PinnedBuf<CrcExtent> h_crc;
+    PinnedBuf<uint32_t> h_piece_base;
+    PinnedBuf<CdcFile> h_files;
+    PinnedBuf<uint64_t> h_rstart, h_rlen;
+    PinnedBuf<uint32_t> h_rstream, h_rflags;
     // device mirrors
-    CrcExtent *d_crc = nullptr;
-    uint32_t *d_piece_base = nullptr;
-    uint32_t *d_ext_pure = nullptr; // pure(extent) of this submit's CRC extents
-    CdcFile *d_files = nullptr;
-    uint64_t *d_rstart = nullptr, *d_rlen = nullptr;
-    uint32_t *d_rstream = nullptr, *d_rflags = nullptr;
-    cudaEvent_t ev_done = nullptr; // kernels that read this set have finished
+    DevBuf<CrcExtent> d_crc;
+    DevBuf<uint32_t> d_piece_base;
+    DevBuf<uint32_t> d_ext_pure; // pure(extent) of this submit's CRC extents
+    DevBuf<CdcFile> d_files;
+    DevBuf<uint64_t> d_rstart, d_rlen;
+    DevBuf<uint32_t> d_rstream, d_rflags;
+    Event ev_done; // kernels that read this set have finished
     bool in_flight = false;
 };
 
 struct HostArena {
-    uint8_t *ptr = nullptr;
-    cudaEvent_t ev_h2d = nullptr;
+    PinnedBuf<uint8_t> ptr;
+    Event ev_h2d;
     bool in_flight = false;
     bool acquired = false;
 };
@@ -81,11 +166,11 @@ struct mksnap {
     CdcParamsDev prm;
     std::string err;
     int sm_count = 132;
-    cudaStream_t s_comp = nullptr, s_copy = nullptr;
+    Stream s_comp, s_copy; // declared first, so destroyed after the buffers and events used on them
 
     uint32_t n_slots = 0;
-    uint8_t *d_slot[MAX_SLOTS] = {nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t ev_slot_free[MAX_SLOTS] = {nullptr, nullptr, nullptr, nullptr};
+    DevBuf<uint8_t> d_slot[MAX_SLOTS];
+    Event ev_slot_free[MAX_SLOTS];
     bool slot_used[MAX_SLOTS] = {false, false, false, false};
 
     std::vector<HostArena> arenas;
@@ -94,32 +179,31 @@ struct mksnap {
     std::vector<MetaSet> meta;
     uint64_t submit_idx = 0;
 
-    CrcConsts *d_consts = nullptr;
-    SessionCounters *d_sc = nullptr;
-    SessionCounters *h_sc = nullptr; // pinned
+    DevBuf<CrcConsts> d_consts;
+    DevBuf<SessionCounters> d_sc;
+    PinnedBuf<SessionCounters> h_sc;
 
-    TileRec *d_tiles = nullptr;
+    DevBuf<TileRec> d_tiles;
     CUtensorMap tm_main[MAX_SLOTS]; // per slot: arena viewed as [rows][128 B]
     CUtensorMap tm_crc[MAX_SLOTS];  // the same with the box of the CRC variant's tiles
-    uint32_t *d_part = nullptr;     // CRC of every 128-byte arena row, written by the CRC variant of the scan
+    DevBuf<uint32_t> d_part;        // CRC of every 128-byte arena row, written by the CRC variant of the scan
     int scan_cfg = 0; // index into SCAN_SHAPES
     bool sha_fma = true; // chunk SHA-256: additions on the FMA pipe
-    uint32_t *d_pool = nullptr;
+    DevBuf<uint32_t> d_pool;
     uint32_t pool_cap = 0;
-    uint32_t *d_pool_count = nullptr;
-    uint32_t *d_counts = nullptr, *d_bases = nullptr;
-    uint32_t *d_scan_tmp = nullptr; // block sums for the generic scan (several levels)
-    uint64_t scan_tmp_words = 0;
+    DevBuf<uint32_t> d_pool_count;
+    DevBuf<uint32_t> d_counts, d_bases;
+    DevBuf<uint32_t> d_scan_tmp; // block sums for the generic scan (several levels)
 
     // session tables
     uint64_t max_chunks = 0;
-    uint64_t *d_chunk_start = nullptr, *d_chunk_len = nullptr, *d_chunk_end = nullptr;
-    uint32_t *d_order = nullptr; // K2 work order of the current batch (batch-relative chunk indices)
+    DevBuf<uint64_t> d_chunk_start, d_chunk_len, d_chunk_end;
+    DevBuf<uint32_t> d_order; // K2 work order of the current batch (batch-relative chunk indices)
     bool sha_order = true;
-    uint8_t *d_digests = nullptr;
+    DevBuf<uint8_t> d_digests;
     uint64_t max_streams = 0;
-    uint8_t *d_stream_digests = nullptr;
-    StreamState *d_stream_state = nullptr;
+    DevBuf<uint8_t> d_stream_digests;
+    DevBuf<StreamState> d_stream_state;
     std::vector<uint32_t> stream_stamp; // submit epoch that last used the stream slot (one piece per stream per submit)
     uint32_t stamp_epoch = 0;
     std::vector<uint8_t> stream_open; // per slot: the last piece carried MKSNAP_R_MORE (finish refuses the session)
@@ -134,33 +218,32 @@ struct mksnap {
         uint32_t stream, more;
     };
     std::vector<LogPiece> log_pending;
-    uint8_t *d_log = nullptr;
-    uint64_t log_cap = 0, log_used = 0;
-    uint64_t *h_flush = nullptr, *d_flush = nullptr; // K4 tables of a flush: start, len (u64), stream, flags (u32)
-    uint64_t flush_cap = 0;                          // rows
-    cudaEvent_t ev_flush = nullptr;                  // the last flush's table copy has left h_flush
+    DevBuf<uint8_t> d_log;
+    uint64_t log_used = 0;
+    PinnedBuf<uint64_t> h_flush; // K4 tables of a flush, 3 words per row: start, len (u64), stream, flags (u32)
+    DevBuf<uint64_t> d_flush;
+    Event ev_flush;              // the last flush's table copy has left h_flush
     bool have_flush_time = false;
     uint64_t crc_bytes = 0;
-    uint32_t *d_crc_session = nullptr; // pure(extent) of every CRC extent of the session, submission order
-    uint64_t crc_session_cap = 0, crc_session_n = 0;
+    DevBuf<uint32_t> d_crc_session; // pure(extent) of every CRC extent of the session, submission order
+    uint64_t crc_session_n = 0;
     uint32_t crc_host_acc = 0;         // contributions folded on the host (mksnap_crc_add)
     uint64_t crc_host_bytes = 0;
-    CrcUse *d_uses = nullptr;          // mksnap_crc_fold: use table (max_extents rows) and stream values (max_streams),
-    uint32_t *d_stream_pure = nullptr; //   allocated by the first fold
+    DevBuf<CrcUse> d_uses;             // mksnap_crc_fold: use table (max_extents rows) and stream values (max_streams),
+    DevBuf<uint32_t> d_stream_pure;    //   allocated by the first fold
     uint64_t fold_streams = 0;         // highest stream slot folded in this session + 1
-    uint8_t *h_add = nullptr;          // mksnap_chunks_add: pinned staging of MKSNAP_CHUNKS_ADD_MAX rows, its device
-    uint8_t *d_add = nullptr;          //   twin and the end of the last copy out of it; allocated by the first call
-    cudaEvent_t ev_add = nullptr;
+    PinnedBuf<uint8_t> h_add;          // mksnap_chunks_add: pinned staging of MKSNAP_CHUNKS_ADD_MAX rows, its device
+    DevBuf<uint8_t> d_add;             //   twin and the end of the last copy out of it; allocated by the first call
+    Event ev_add;
     bool open_file = false;      // the last submit ended with a MKSNAP_X_MORE extent: the next must start with its continuation
-    uint8_t *d_carry = nullptr;  // open chunk of that file (k_carry_out -> k_carry_in)
-    uint64_t carry_cap = 0;
+    DevBuf<uint8_t> d_carry;     // open chunk of that file (k_carry_out -> k_carry_in)
 
     // sort / table
-    uint64_t *d_keys[2] = {nullptr, nullptr};
-    uint32_t *d_idx[2] = {nullptr, nullptr};
-    uint8_t *d_sorted = nullptr, *d_table = nullptr;
-    uint32_t *d_flags = nullptr, *d_pos = nullptr, *d_hist = nullptr;
-    uint8_t *d_merkle[2] = {nullptr, nullptr};
+    DevBuf<uint64_t> d_keys[2];
+    DevBuf<uint32_t> d_idx[2];
+    DevBuf<uint8_t> d_sorted, d_table;
+    DevBuf<uint32_t> d_flags, d_pos, d_hist;
+    DevBuf<uint8_t> d_merkle[2];
     uint64_t table_cap = 0; // rows the sort buffers can hold
     uint64_t n_unique = 0;
     uint8_t root[32];
@@ -172,22 +255,20 @@ struct mksnap {
     NcclApi nccl;
     void *comm = nullptr;
     int n_ranks = 1, rank = 0;
-    uint8_t *d_gather = nullptr; // n_ranks * pad_rows * 32
-    uint64_t gather_rows = 0;
-    unsigned long long *d_gcount = nullptr; // n_ranks * GH_WORDS header words
-    uint8_t *d_concat = nullptr;            // dense concatenation of all ranks' tables
-    uint64_t concat_rows = 0;
+    DevBuf<uint8_t> d_gather;                // n_ranks * pad_rows * 32
+    DevBuf<unsigned long long> d_gcount;     // n_ranks * GH_WORDS header words
+    DevBuf<uint8_t> d_concat;                // dense concatenation of all ranks' tables
     // range-partitioned exchange (mksnap_exchange_tables): small fixed-size scratch
-    unsigned long long *d_xbounds = nullptr; // R+1 slice boundaries of my table
-    unsigned long long *d_xhdr = nullptr;    // R * (GH_WORDS + R) header words
-    uint8_t *d_xrec = nullptr;               // R records of XREC_BYTES: u64 rows-in-range, then the first 255 rows
-    uint8_t *d_xtail = nullptr;              // 256 rows: the Merkle group that straddles the end of my range
-    int x_ranks = 0;
+    DevBuf<unsigned long long> d_xbounds;    // R+1 slice boundaries of my table
+    DevBuf<unsigned long long> d_xhdr;       // R * (GH_WORDS + R) header words
+    DevBuf<uint8_t> d_xrec;                  // R records of XREC_BYTES: u64 rows-in-range, then the first 255 rows
+    DevBuf<uint8_t> d_xtail;                 // 256 rows: the Merkle group that straddles the end of my range
+    int x_ranks = 0;                         // ranks the four buffers above hold
 
     // timing
-    cudaEvent_t ev[N_EV];
-    cudaEvent_t ev_copy0 = nullptr, ev_copy1 = nullptr, ev_copy_done = nullptr;
-    cudaEvent_t ev_fin[4];
+    Event ev[N_EV];
+    Event ev_copy0, ev_copy1, ev_copy_done;
+    Event ev_fin[4];
     bool have_submit_times = false, have_h2d_time = false, have_fin_times = false, have_gather_time = false;
     mksnap_stats_t stats;
 
@@ -283,9 +364,9 @@ int scan_u32(mksnap *h, const uint32_t *in, uint32_t *out, uint64_t n, cudaStrea
         off[l] = total;
         total += sizes[l];
     }
-    if (total > h->scan_tmp_words)
+    if (total > h->d_scan_tmp.size())
         return fail(h, MKSNAP_E_CAPACITY, "scan temp too small (%llu > %llu)", (unsigned long long)total,
-                    (unsigned long long)h->scan_tmp_words);
+                    (unsigned long long)h->d_scan_tmp.size());
     // up-sweep: reduce each level into the next
     for (size_t l = 0; l + 1 < sizes.size(); l++) {
         const uint32_t *src = l == 0 ? in : h->d_scan_tmp + off[l];
@@ -335,7 +416,7 @@ int sort_unique_root(mksnap *h, const uint8_t *src, uint64_t n, cudaStream_t s)
         k_gather_digests<<<(uint32_t)((2 * n + tb - 1) / tb), tb, 0, s>>>(src, h->d_idx[cur], n, h->d_sorted);
         LAUNCH_OK(h);
         // long runs (duplicates) are listed in the idle flag buffer and handled by whole CTAs
-        uint2 *long_runs = reinterpret_cast<uint2 *>(h->d_hist); // sized for FIX_LONG_CAP entries in alloc_table_buffers
+        uint2 *long_runs = reinterpret_cast<uint2 *>(h->d_hist.get()); // sized for FIX_LONG_CAP entries in alloc_table_buffers
         uint32_t *n_long = h->d_pos;
         CK(h, cudaMemsetAsync(n_long, 0, 4, s));
         k_fix_ties<<<(uint32_t)((n + tb - 1) / tb), tb, 0, s>>>(h->d_keys[cur], n, h->d_sorted, 64 - SORT_KEY_BITS, long_runs, n_long);
@@ -431,30 +512,21 @@ static int make_row_map(mksnap *h, EncodeTiledFn enc, CUtensorMap *out, void *ba
 // and again by mksnap_comm_init (rows = max_chunks x ranks: every rank merges the union of all tables).
 static int alloc_table_buffers(mksnap *h, uint64_t rows)
 {
-    for (int k = 0; k < 2; k++) {
-        cudaFree(h->d_keys[k]); cudaFree(h->d_idx[k]); cudaFree(h->d_merkle[k]);
-        h->d_keys[k] = nullptr; h->d_idx[k] = nullptr; h->d_merkle[k] = nullptr;
-    }
-    cudaFree(h->d_sorted); cudaFree(h->d_table); cudaFree(h->d_flags); cudaFree(h->d_pos); cudaFree(h->d_hist);
-    cudaFree(h->d_scan_tmp);
-    h->d_sorted = h->d_table = nullptr;
-    h->d_flags = h->d_pos = h->d_hist = h->d_scan_tmp = nullptr;
     h->table_cap = 0;
     for (int k = 0; k < 2; k++) {
-        CK(h, cudaMalloc(&h->d_keys[k], rows * 8));
-        CK(h, cudaMalloc(&h->d_idx[k], rows * 4));
+        CK(h, h->d_keys[k].alloc(rows));
+        CK(h, h->d_idx[k].alloc(rows));
     }
-    CK(h, cudaMalloc(&h->d_sorted, rows * 32));
-    CK(h, cudaMalloc(&h->d_table, rows * 32));
-    CK(h, cudaMalloc(&h->d_flags, rows * 4));
-    CK(h, cudaMalloc(&h->d_pos, rows * 4));
+    CK(h, h->d_sorted.alloc(rows * 32));
+    CK(h, h->d_table.alloc(rows * 32));
+    CK(h, h->d_flags.alloc(rows));
+    CK(h, h->d_pos.alloc(rows));
     const uint64_t hist_words = std::max<uint64_t>(256ull * ((rows + SORT_TILE - 1) / SORT_TILE + 1), 2ull * FIX_LONG_CAP + 64); // also holds k_fix_ties' long-run list
-    CK(h, cudaMalloc(&h->d_hist, hist_words * 4));
+    CK(h, h->d_hist.alloc(hist_words));
     const uint64_t merkle_rows = rows / 256 + 2;
-    CK(h, cudaMalloc(&h->d_merkle[0], merkle_rows * 32));
-    CK(h, cudaMalloc(&h->d_merkle[1], (merkle_rows / 256 + 2) * 32));
-    h->scan_tmp_words = std::max(rows, std::max<uint64_t>(hist_words, h->cfg.max_extents)) / SCAN_ITEMS * 2 + 4096;
-    CK(h, cudaMalloc(&h->d_scan_tmp, h->scan_tmp_words * 4));
+    CK(h, h->d_merkle[0].alloc(merkle_rows * 32));
+    CK(h, h->d_merkle[1].alloc((merkle_rows / 256 + 2) * 32));
+    CK(h, h->d_scan_tmp.alloc(std::max(rows, std::max<uint64_t>(hist_words, h->cfg.max_extents)) / SCAN_ITEMS * 2 + 4096));
     h->table_cap = rows;
     return 0;
 }
@@ -517,55 +589,55 @@ static int create_impl(mksnap *h)
         return fail(h, MKSNAP_E_CUDA, "device %d is sm_%d%d; libmksnap is built for sm_90a only", c.device,
                     prop.major, prop.minor);
     h->sm_count = prop.multiProcessorCount;
-    CK(h, cudaStreamCreateWithFlags(&h->s_comp, cudaStreamNonBlocking));
-    CK(h, cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking));
+    CK(h, cudaStreamCreateWithFlags(h->s_comp.put(), cudaStreamNonBlocking));
+    CK(h, cudaStreamCreateWithFlags(h->s_copy.put(), cudaStreamNonBlocking));
 
     h->n_slots = c.n_device_slots ? c.n_device_slots : (c.n_host_arenas ? 2u : 1u);
     if (h->n_slots > MAX_SLOTS)
         return fail(h, MKSNAP_E_INVAL, "n_device_slots > %u", MAX_SLOTS);
     for (uint32_t s = 0; s < h->n_slots; s++) {
-        CK(h, cudaMalloc(&h->d_slot[s], c.device_arena_bytes + SLOT_SLACK));
+        CK(h, h->d_slot[s].alloc(c.device_arena_bytes + SLOT_SLACK));
         CK(h, cudaMemsetAsync(h->d_slot[s] + c.device_arena_bytes, 0, SLOT_SLACK, h->s_comp));
-        CK(h, cudaEventCreateWithFlags(&h->ev_slot_free[s], cudaEventDisableTiming));
+        CK(h, cudaEventCreateWithFlags(h->ev_slot_free[s].put(), cudaEventDisableTiming));
     }
     h->arenas.resize(c.n_host_arenas);
     for (auto &a : h->arenas) {
-        CK(h, cudaHostAlloc(&a.ptr, c.host_arena_bytes, cudaHostAllocDefault));
-        CK(h, cudaEventCreateWithFlags(&a.ev_h2d, cudaEventDisableTiming));
+        CK(h, a.ptr.alloc(c.host_arena_bytes));
+        CK(h, cudaEventCreateWithFlags(a.ev_h2d.put(), cudaEventDisableTiming));
     }
     const uint64_t mx = c.max_extents;
     h->meta.resize(std::max<uint32_t>(2, h->n_slots));
     for (auto &m : h->meta) {
-        CK(h, cudaHostAlloc(&m.h_crc, mx * sizeof(CrcExtent), cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_piece_base, (mx + 1) * 4, cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_files, mx * sizeof(CdcFile), cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_rstart, mx * 8, cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_rlen, mx * 8, cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_rstream, mx * 4, cudaHostAllocDefault));
-        CK(h, cudaHostAlloc(&m.h_rflags, mx * 4, cudaHostAllocDefault));
-        CK(h, cudaMalloc(&m.d_crc, mx * sizeof(CrcExtent)));
-        CK(h, cudaMalloc(&m.d_piece_base, (mx + 1) * 4));
-        CK(h, cudaMalloc(&m.d_ext_pure, mx * 4));
-        CK(h, cudaMalloc(&m.d_files, mx * sizeof(CdcFile)));
-        CK(h, cudaMalloc(&m.d_rstart, mx * 8));
-        CK(h, cudaMalloc(&m.d_rlen, mx * 8));
-        CK(h, cudaMalloc(&m.d_rstream, mx * 4));
-        CK(h, cudaMalloc(&m.d_rflags, mx * 4));
-        CK(h, cudaEventCreateWithFlags(&m.ev_done, cudaEventDisableTiming));
+        CK(h, m.h_crc.alloc(mx));
+        CK(h, m.h_piece_base.alloc(mx + 1));
+        CK(h, m.h_files.alloc(mx));
+        CK(h, m.h_rstart.alloc(mx));
+        CK(h, m.h_rlen.alloc(mx));
+        CK(h, m.h_rstream.alloc(mx));
+        CK(h, m.h_rflags.alloc(mx));
+        CK(h, m.d_crc.alloc(mx));
+        CK(h, m.d_piece_base.alloc(mx + 1));
+        CK(h, m.d_ext_pure.alloc(mx));
+        CK(h, m.d_files.alloc(mx));
+        CK(h, m.d_rstart.alloc(mx));
+        CK(h, m.d_rlen.alloc(mx));
+        CK(h, m.d_rstream.alloc(mx));
+        CK(h, m.d_rflags.alloc(mx));
+        CK(h, cudaEventCreateWithFlags(m.ev_done.put(), cudaEventDisableTiming));
     }
 
     CrcConsts *hc = new CrcConsts;
     build_crc_consts(hc);
-    CK(h, cudaMalloc(&h->d_consts, sizeof(CrcConsts)));
+    CK(h, h->d_consts.alloc(1));
     CK(h, cudaMemcpy(h->d_consts, hc, sizeof(CrcConsts), cudaMemcpyHostToDevice));
     delete hc;
-    CK(h, cudaMalloc(&h->d_sc, sizeof(SessionCounters)));
+    CK(h, h->d_sc.alloc(1));
     CK(h, cudaMemset(h->d_sc, 0, sizeof(SessionCounters)));
-    CK(h, cudaHostAlloc(&h->h_sc, sizeof(SessionCounters), cudaHostAllocDefault));
+    CK(h, h->h_sc.alloc(1));
 
     const uint64_t n_tiles = c.device_arena_bytes / SCAN_TILE + 128; // one TileRec per 4 KiB region (+ tile round-up)
-    CK(h, cudaMalloc(&h->d_tiles, n_tiles * sizeof(TileRec)));
-    CK(h, cudaMalloc(&h->d_part, n_tiles * (SCAN_TILE / CRC_GRANULE) * 4)); // one u32 per row of every scanned region
+    CK(h, h->d_tiles.alloc(n_tiles));
+    CK(h, h->d_part.alloc(n_tiles * (SCAN_TILE / CRC_GRANULE))); // one u32 per row of every scanned region
     {
         EncodeTiledFn enc = nullptr;
         cudaDriverEntryPointQueryResult qres;
@@ -604,32 +676,30 @@ static int create_impl(mksnap *h)
     if (pc > 0xFFFFFFF0ull)
         pc = 0xFFFFFFF0ull;
     h->pool_cap = (uint32_t)pc;
-    CK(h, cudaMalloc(&h->d_pool, (uint64_t)h->pool_cap * 4));
-    CK(h, cudaMalloc(&h->d_pool_count, 4));
-    h->crc_session_cap = std::max<uint64_t>(4 * mx, 1ull << 20);
-    CK(h, cudaMalloc(&h->d_crc_session, h->crc_session_cap * 4));
-    h->carry_cap = ((uint64_t)h->prm.max_size + 511) / 512 * 512;
-    CK(h, cudaMalloc(&h->d_carry, h->carry_cap));
-    CK(h, cudaMalloc(&h->d_counts, mx * 4));
-    CK(h, cudaMalloc(&h->d_bases, mx * 4));
+    CK(h, h->d_pool.alloc(h->pool_cap));
+    CK(h, h->d_pool_count.alloc(1));
+    CK(h, h->d_crc_session.alloc(std::max<uint64_t>(4 * mx, 1ull << 20)));
+    CK(h, h->d_carry.alloc(((uint64_t)h->prm.max_size + 511) / 512 * 512));
+    CK(h, h->d_counts.alloc(mx));
+    CK(h, h->d_bases.alloc(mx));
 
     // default: every byte in min-size chunks, plus per file the end-of-file chunk and the two spare cut-list slots of the big-file path
     h->max_chunks = c.max_chunks ? c.max_chunks : c.device_arena_bytes / h->prm.min_size + 3 * mx + 64;
     const uint64_t mc = h->max_chunks;
-    CK(h, cudaMalloc(&h->d_chunk_start, mc * 8));
-    CK(h, cudaMalloc(&h->d_chunk_len, mc * 8));
-    CK(h, cudaMalloc(&h->d_order, mc * 4));
-    CK(h, cudaMalloc(&h->d_chunk_end, mc * 8));
-    CK(h, cudaMalloc(&h->d_digests, mc * 32));
+    CK(h, h->d_chunk_start.alloc(mc));
+    CK(h, h->d_chunk_len.alloc(mc));
+    CK(h, h->d_order.alloc(mc));
+    CK(h, h->d_chunk_end.alloc(mc));
+    CK(h, h->d_digests.alloc(mc * 32));
     h->max_streams = mx;
-    CK(h, cudaMalloc(&h->d_stream_digests, h->max_streams * 32));
-    CK(h, cudaMalloc(&h->d_stream_state, h->max_streams * sizeof(StreamState)));
+    CK(h, h->d_stream_digests.alloc(h->max_streams * 32));
+    CK(h, h->d_stream_state.alloc(h->max_streams));
     CK(h, cudaMemset(h->d_stream_state, 0, h->max_streams * sizeof(StreamState)));
     h->stream_stamp.assign(h->max_streams, 0);
     h->stream_open.assign(h->max_streams, 0);
     h->stream_defer.assign(h->max_streams, 0);
     h->log_count.assign(h->max_streams, 0);
-    CK(h, cudaEventCreateWithFlags(&h->ev_flush, cudaEventDisableTiming));
+    CK(h, cudaEventCreateWithFlags(h->ev_flush.put(), cudaEventDisableTiming));
 
     {
         int rc = alloc_table_buffers(h, mc);
@@ -638,12 +708,12 @@ static int create_impl(mksnap *h)
     }
 
     for (int i = 0; i < N_EV; i++)
-        CK(h, cudaEventCreate(&h->ev[i]));
+        CK(h, cudaEventCreate(h->ev[i].put()));
     for (int i = 0; i < 4; i++)
-        CK(h, cudaEventCreate(&h->ev_fin[i]));
-    CK(h, cudaEventCreate(&h->ev_copy0));
-    CK(h, cudaEventCreate(&h->ev_copy1));
-    CK(h, cudaEventCreateWithFlags(&h->ev_copy_done, cudaEventDisableTiming));
+        CK(h, cudaEventCreate(h->ev_fin[i].put()));
+    CK(h, cudaEventCreate(h->ev_copy0.put()));
+    CK(h, cudaEventCreate(h->ev_copy1.put()));
+    CK(h, cudaEventCreateWithFlags(h->ev_copy_done.put(), cudaEventDisableTiming));
     CK(h, cudaFuncSetAttribute(k_crc32_extents, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CRC_SMEM));
     CK(h, cudaFuncSetAttribute(k_select_cuts_big, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SELB_SMEM));
     CK(h, cudaStreamSynchronize(h->s_comp));
@@ -701,48 +771,7 @@ void mksnap_destroy(mksnap_t *h)
     gz_free(h);
     if (h->comm && h->nccl.CommDestroy)
         h->nccl.CommDestroy(h->comm);
-    for (uint32_t s = 0; s < MAX_SLOTS; s++) {
-        cudaFree(h->d_slot[s]);
-        if (h->ev_slot_free[s])
-            cudaEventDestroy(h->ev_slot_free[s]);
-    }
-    for (auto &a : h->arenas) {
-        cudaFreeHost(a.ptr);
-        if (a.ev_h2d)
-            cudaEventDestroy(a.ev_h2d);
-    }
-    for (auto &m : h->meta) {
-        cudaFreeHost(m.h_crc); cudaFreeHost(m.h_piece_base); cudaFreeHost(m.h_files);
-        cudaFreeHost(m.h_rstart); cudaFreeHost(m.h_rlen); cudaFreeHost(m.h_rstream); cudaFreeHost(m.h_rflags);
-        cudaFree(m.d_rstream); cudaFree(m.d_rflags);
-        cudaFree(m.d_ext_pure);
-        cudaFree(m.d_crc); cudaFree(m.d_piece_base); cudaFree(m.d_files); cudaFree(m.d_rstart); cudaFree(m.d_rlen);
-        if (m.ev_done)
-            cudaEventDestroy(m.ev_done);
-    }
-    cudaFree(h->d_consts); cudaFree(h->d_sc); cudaFreeHost(h->h_sc);
-    cudaFree(h->d_carry);
-    cudaFree(h->d_crc_session);
-    cudaFree(h->d_uses); cudaFree(h->d_stream_pure);
-    cudaFreeHost(h->h_add); cudaFree(h->d_add);
-    if (h->ev_add)
-        cudaEventDestroy(h->ev_add);
-    cudaFree(h->d_tiles); cudaFree(h->d_part); cudaFree(h->d_pool); cudaFree(h->d_pool_count); cudaFree(h->d_counts); cudaFree(h->d_bases);
-    cudaFree(h->d_scan_tmp);
-    cudaFree(h->d_order); cudaFree(h->d_chunk_start); cudaFree(h->d_chunk_len); cudaFree(h->d_chunk_end); cudaFree(h->d_digests);
-    cudaFree(h->d_stream_digests); cudaFree(h->d_stream_state);
-    cudaFree(h->d_log); cudaFree(h->d_flush); cudaFreeHost(h->h_flush);
-    if (h->ev_flush)
-        cudaEventDestroy(h->ev_flush);
-    for (int k = 0; k < 2; k++) {
-        cudaFree(h->d_keys[k]); cudaFree(h->d_idx[k]); cudaFree(h->d_merkle[k]);
-    }
-    cudaFree(h->d_sorted); cudaFree(h->d_table); cudaFree(h->d_flags); cudaFree(h->d_pos); cudaFree(h->d_hist);
-    cudaFree(h->d_gather); cudaFree(h->d_gcount); cudaFree(h->d_concat);
-    cudaFree(h->d_xbounds); cudaFree(h->d_xhdr); cudaFree(h->d_xrec); cudaFree(h->d_xtail);
-    if (h->s_comp) cudaStreamDestroy(h->s_comp);
-    if (h->s_copy) cudaStreamDestroy(h->s_copy);
-    delete h;
+    delete h; // the members free the buffers, events and streams
 }
 
 int mksnap_begin(mksnap_t *h)
@@ -827,7 +856,7 @@ int mksnap_get_limits(const mksnap_t *h, mksnap_limits *out)
     out->device_arena_bytes = h->cfg.device_arena_bytes;
     out->n_host_arenas = (uint32_t)h->arenas.size();
     out->n_device_slots = h->n_slots;
-    out->carry_bytes = h->carry_cap;
+    out->carry_bytes = h->d_carry.size();
     return 0;
 }
 
@@ -849,19 +878,13 @@ int mksnap_reserve_stream_log(mksnap_t *h, uint64_t bytes)
                     (unsigned long long)h->log_pending.size());
     CK(h, cudaSetDevice(h->cfg.device));
     bytes = (bytes + 63) & ~63ull; // K4 reads a piece's last block in whole 16-byte words
-    if (bytes == h->log_cap)
+    if (bytes == h->d_log.size())
         return 0;
     CK(h, cudaStreamSynchronize(h->s_comp));
-    CK(h, cudaFree(h->d_log));
-    h->d_log = nullptr;
-    h->log_cap = 0;
-    if (bytes) {
-        if (cudaMalloc(&h->d_log, bytes) != cudaSuccess) {
-            cudaGetLastError();
-            h->d_log = nullptr;
-            return fail(h, MKSNAP_E_NOMEM, "stream log of %llu bytes", (unsigned long long)bytes);
-        }
-        h->log_cap = bytes;
+    h->d_log.reset();
+    if (bytes && h->d_log.alloc(bytes) != cudaSuccess) {
+        cudaGetLastError();
+        return fail(h, MKSNAP_E_NOMEM, "stream log of %llu bytes", (unsigned long long)bytes);
     }
     return 0;
 }
@@ -900,16 +923,11 @@ static int flush_log(mksnap *h, cudaStream_t sk)
         groups.push_back(Group{p.off, p.len, p.stream, p.more, round});
     }
     const uint64_t n = groups.size();
-    if (n > h->flush_cap) {
+    if (n * 3 > std::min(h->h_flush.size(), h->d_flush.size())) { // either is empty after a failed growth
         CK(h, cudaStreamSynchronize(sk));
-        CK(h, cudaFreeHost(h->h_flush));
-        CK(h, cudaFree(h->d_flush));
-        h->h_flush = h->d_flush = nullptr;
-        h->flush_cap = 0;
         const uint64_t cap = std::max<uint64_t>(n, 1024);
-        CK(h, cudaHostAlloc(&h->h_flush, cap * 24, cudaHostAllocDefault));
-        CK(h, cudaMalloc(&h->d_flush, cap * 24));
-        h->flush_cap = cap;
+        CK(h, h->h_flush.alloc(cap * 3));
+        CK(h, h->d_flush.alloc(cap * 3));
     } else {
         CK(h, cudaEventSynchronize(h->ev_flush));
     }
@@ -992,9 +1010,9 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
                 if (n_files != 0 || !h->open_file)
                     return fail(h, MKSNAP_E_STATE, "extent %llu: MKSNAP_X_CONT must be the first CDC extent of the submit that follows a MKSNAP_X_MORE extent",
                                 (unsigned long long)i);
-                if (x.arena_off < h->carry_cap)
+                if (x.arena_off < h->d_carry.size())
                     return fail(h, MKSNAP_E_INVAL, "extent %llu: a continuation starts at arena offset >= %llu (room for the open chunk)",
-                                (unsigned long long)i, (unsigned long long)h->carry_cap);
+                                (unsigned long long)i, (unsigned long long)h->d_carry.size());
                 have_cont = true;
                 cont_off = x.arena_off;
             }
@@ -1011,8 +1029,8 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
             m.h_files[n_files].scratch = big_slots;
             m.h_files[n_files].more_after = more ? x.reserved : 0u;
             m.h_files[n_files].cont = cont ? 1u : 0u;
-            if (x.len + (cont ? h->carry_cap : 0) >= SELECT_BIG_FILE) // a continuation is widened by its open chunk on the device
-                big_slots += (x.len + (cont ? h->carry_cap : 0)) / h->prm.min_size + 2;
+            if (x.len + (cont ? h->d_carry.size() : 0) >= SELECT_BIG_FILE) // a continuation is widened by its open chunk on the device
+                big_slots += (x.len + (cont ? h->d_carry.size() : 0)) / h->prm.min_size + 2;
             cdc_bytes += x.len;
             n_files++;
         } else if (x.flags & (MKSNAP_X_MORE | MKSNAP_X_CONT)) {
@@ -1051,7 +1069,7 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
     std::vector<uint64_t> logged;
     uint64_t n_inline = 0;
     for (uint64_t i = 0; i < n_rng; i++) {
-        if ((rng[i].flags & MKSNAP_R_DEFER) && h->log_cap && rng[i].len <= h->log_cap) {
+        if ((rng[i].flags & MKSNAP_R_DEFER) && h->d_log.size() && rng[i].len <= h->d_log.size()) {
             logged.push_back(i);
             continue;
         }
@@ -1129,15 +1147,15 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         CK(h, cudaMemsetAsync(m.d_ext_pure, 0, n_crc * 4, sk));
         k_crc32_extents<<<grid, CRC_THREADS, CRC_SMEM, sk>>>(d_arena, m.d_crc, m.d_piece_base, (uint32_t)n_crc,
                                                             (uint32_t)pieces, h->d_consts, m.d_ext_pure, &h->d_sc->crc_acc,
-                                                            n_files ? h->d_part : nullptr);
+                                                            n_files ? h->d_part.get() : nullptr);
         LAUNCH_OK(h);
     }
     if (n_crc) { // pure(extent) of this submit's extents joins the session table (zero-length extents keep their slot)
         if (!pieces)
             CK(h, cudaMemsetAsync(m.d_ext_pure, 0, n_crc * 4, sk));
-        if (h->crc_session_n < h->crc_session_cap)
+        if (h->crc_session_n < h->d_crc_session.size())
             CK(h, cudaMemcpyAsync(h->d_crc_session + h->crc_session_n, m.d_ext_pure,
-                                  std::min<uint64_t>(n_crc, h->crc_session_cap - h->crc_session_n) * 4, cudaMemcpyDeviceToDevice, sk));
+                                  std::min<uint64_t>(n_crc, h->d_crc_session.size() - h->crc_session_n) * 4, cudaMemcpyDeviceToDevice, sk));
         h->crc_session_n += n_crc;
     }
     CK(h, cudaEventRecord(h->ev[2], sk));
@@ -1188,7 +1206,7 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
         k_batch_end<<<1, 32, 0, sk>>>(h->d_sc);
         LAUNCH_OK(h);
         if (have_more) { // park the open chunk before this slot is recycled
-            k_carry_out<<<1, 256, 0, sk>>>(d_arena, h->d_carry, h->carry_cap, h->d_sc);
+            k_carry_out<<<1, 256, 0, sk>>>(d_arena, h->d_carry, h->d_carry.size(), h->d_sc);
             LAUNCH_OK(h);
         }
     }
@@ -1196,7 +1214,7 @@ static int submit_common(mksnap *h, uint32_t slot, uint64_t used, const mksnap_e
     for (const uint64_t i : logged) { // into the log before the slot is recycled; a full log is hashed first
         const mksnap_range &r = rng[i];
         uint64_t off = (h->log_used + 15) & ~15ull;
-        if (off + r.len > h->log_cap) {
+        if (off + r.len > h->d_log.size()) {
             int rc = flush_log(h, sk);
             if (rc)
                 return rc;
@@ -1311,10 +1329,10 @@ int mksnap_chunks_add(mksnap_t *h, const uint8_t *digests, uint64_t n)
         return 0;
     CK(h, cudaSetDevice(h->cfg.device));
     cudaStream_t s = h->s_comp; // behind the submits enqueued before this call
-    if (!h->h_add) {
-        CK(h, cudaHostAlloc(&h->h_add, (uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32, cudaHostAllocDefault));
-        CK(h, cudaMalloc(&h->d_add, (uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32));
-        CK(h, cudaEventCreateWithFlags(&h->ev_add, cudaEventDisableTiming));
+    if (!h->ev_add) { // created last: a first call that failed part-way allocates again
+        CK(h, h->h_add.alloc((uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32));
+        CK(h, h->d_add.alloc((uint64_t)MKSNAP_CHUNKS_ADD_MAX * 32));
+        CK(h, cudaEventCreateWithFlags(h->ev_add.put(), cudaEventDisableTiming));
     } else {
         CK(h, cudaEventSynchronize(h->ev_add)); // the previous call's copy has left the staging buffer
     }
@@ -1323,8 +1341,8 @@ int mksnap_chunks_add(mksnap_t *h, const uint8_t *digests, uint64_t n)
     CK(h, cudaEventRecord(h->ev_add, s));
     h->stats.h2d_bytes += n * 32;
     const uint32_t grid = (uint32_t)std::min<uint64_t>((2 * n + APPEND_THREADS - 1) / APPEND_THREADS, (uint64_t)h->sm_count * 4);
-    k_chunks_append<<<grid, APPEND_THREADS, 0, s>>>(reinterpret_cast<const uint4 *>(h->d_add), (uint32_t)n, h->d_sc,
-                                                    h->max_chunks, reinterpret_cast<uint4 *>(h->d_digests), h->d_chunk_end);
+    k_chunks_append<<<grid, APPEND_THREADS, 0, s>>>(reinterpret_cast<const uint4 *>(h->d_add.get()), (uint32_t)n, h->d_sc,
+                                                    h->max_chunks, reinterpret_cast<uint4 *>(h->d_digests.get()), h->d_chunk_end);
     LAUNCH_OK(h);
     k_chunks_commit<<<1, 32, 0, s>>>(h->d_sc, (uint32_t)n, h->max_chunks);
     LAUNCH_OK(h);
@@ -1503,9 +1521,9 @@ int mksnap_get_extent_crcs(mksnap_t *h, uint32_t *pure, uint64_t capacity, uint6
         return h ? fail(h, MKSNAP_E_STATE, "get_extent_crcs before finish") : MKSNAP_E_INVAL;
     CK(h, cudaSetDevice(h->cfg.device));
     *n_out = h->crc_session_n;
-    if (h->crc_session_n > h->crc_session_cap)
+    if (h->crc_session_n > h->d_crc_session.size())
         return fail(h, MKSNAP_E_CAPACITY, "the session submitted %llu CRC extents, the per-extent table keeps %llu",
-                    (unsigned long long)h->crc_session_n, (unsigned long long)h->crc_session_cap);
+                    (unsigned long long)h->crc_session_n, (unsigned long long)h->d_crc_session.size());
     if (!pure || h->crc_session_n > capacity)
         return fail(h, MKSNAP_E_CAPACITY, "need %llu entries", (unsigned long long)h->crc_session_n);
     if (h->crc_session_n)
@@ -1527,9 +1545,9 @@ int mksnap_crc_fold(mksnap_t *h, const mksnap_crc_use *uses, uint64_t n)
     if (n > h->cfg.max_extents)
         return fail(h, MKSNAP_E_CAPACITY, "crc_fold: %llu uses in one call, max_extents is %llu", (unsigned long long)n,
                     (unsigned long long)h->cfg.max_extents);
-    if (h->crc_session_n > h->crc_session_cap)
+    if (h->crc_session_n > h->d_crc_session.size())
         return fail(h, MKSNAP_E_CAPACITY, "crc_fold: the session submitted %llu CRC extents, the per-extent table keeps %llu",
-                    (unsigned long long)h->crc_session_n, (unsigned long long)h->crc_session_cap);
+                    (unsigned long long)h->crc_session_n, (unsigned long long)h->d_crc_session.size());
     uint64_t hi = 0;
     for (uint64_t i = 0; i < n; i++) {
         const mksnap_crc_use &u = uses[i];
@@ -1547,9 +1565,9 @@ int mksnap_crc_fold(mksnap_t *h, const mksnap_crc_use *uses, uint64_t n)
         return 0;
     CK(h, cudaSetDevice(h->cfg.device));
     cudaStream_t s = h->s_comp; // after the K0 runs and the d_crc_session copies the uses read
-    if (!h->d_uses) {
-        CK(h, cudaMalloc(&h->d_uses, h->cfg.max_extents * sizeof(CrcUse)));
-        CK(h, cudaMalloc(&h->d_stream_pure, h->max_streams * 4));
+    if (!h->d_stream_pure) { // allocated last: a first call that failed part-way allocates again
+        CK(h, h->d_uses.alloc(h->cfg.max_extents));
+        CK(h, h->d_stream_pure.alloc(h->max_streams));
         CK(h, cudaMemsetAsync(h->d_stream_pure, 0, h->max_streams * 4, s));
     }
     CK(h, cudaMemcpyAsync(h->d_uses, uses, n * sizeof(CrcUse), cudaMemcpyHostToDevice, s));

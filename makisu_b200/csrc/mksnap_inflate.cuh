@@ -187,22 +187,22 @@ struct Window {
 } // namespace gz
 
 struct mksnap_gunzip_state {
-    uint8_t *d_gz = nullptr;
+    Stream s; // the gunzip's own stream: window decodes do not queue behind an open ingest session (declared first, so
+              // destroyed after the buffers and events used on it)
+    DevBuf<uint8_t> d_gz;
     uint64_t gz_len = 0;
-    uint64_t *d_cand = nullptr;
+    DevBuf<uint64_t> d_cand;
     uint64_t n_cand = 0;
-    mki::SegRes *d_res = nullptr;
-    mki::Seg *d_segs = nullptr;
-    uint64_t *d_seg_off = nullptr;
-    uint16_t *d_sym = nullptr;
-    uint8_t *d_out = nullptr;
-    uint8_t *h_out = nullptr; // pinned copy of the decoded window: reads are host copies, one D2H per window
-    uint8_t *d_hist[2] = {nullptr, nullptr};
-    cudaStream_t s = nullptr; // the gunzip's own stream: window decodes do not queue behind an open ingest session
+    DevBuf<mki::SegRes> d_res;
+    DevBuf<mki::Seg> d_segs;
+    DevBuf<uint64_t> d_seg_off;
+    DevBuf<uint16_t> d_sym;
+    DevBuf<uint8_t> d_out;
+    PinnedBuf<uint8_t> h_out; // pinned copy of the decoded window: reads are host copies, one D2H per window
+    DevBuf<uint8_t> d_hist[2];
     int hist_cur = 0;
-    CrcExtent *d_ext = nullptr;
-    uint32_t *d_pb = nullptr, *d_pure = nullptr, *d_bad = nullptr; // piece bases, pure(extent), flags
-    uint64_t ext_cap = 0;
+    DevBuf<CrcExtent> d_ext;
+    DevBuf<uint32_t> d_pb, d_pure, d_bad; // piece bases, pure(extent), flags
     std::vector<mki::Seg> segs;
     std::vector<mki::Member> mems;
     std::vector<gz::Window> wins;
@@ -215,8 +215,8 @@ struct mksnap_gunzip_state {
     bool indexed = false;           // opened by mksnap_gunzip_open_indexed: bit positions, k_gz_decode_bits
     std::vector<uint64_t> index;    // ... and the points mksnap_gunzip_get_index returns
     mksnap_gunzip_index_info idx{};
-    mksnap_gunzip_times times;
-    cudaEvent_t ev[6];
+    mksnap_gunzip_times times{};
+    Event ev[6];
 };
 
 namespace {
@@ -226,17 +226,8 @@ void gz_free(mksnap *h)
     mksnap_gunzip_state *g = h->gz;
     if (!g)
         return;
-    if (g->s) {
+    if (g->s)
         cudaStreamSynchronize(g->s);
-        cudaStreamDestroy(g->s);
-    }
-    cudaFreeHost(g->h_out);
-    cudaFree(g->d_gz); cudaFree(g->d_cand); cudaFree(g->d_res); cudaFree(g->d_segs); cudaFree(g->d_seg_off);
-    cudaFree(g->d_sym); cudaFree(g->d_out); cudaFree(g->d_hist[0]); cudaFree(g->d_hist[1]);
-    cudaFree(g->d_ext); cudaFree(g->d_pb); cudaFree(g->d_pure); cudaFree(g->d_bad);
-    for (cudaEvent_t e : g->ev)
-        if (e)
-            cudaEventDestroy(e);
     delete g;
     h->gz = nullptr;
 }
@@ -248,12 +239,6 @@ float gz_ms(mksnap_gunzip_state *g, int a, int b)
     return t;
 }
 
-// device scratch of one call, freed on every return path
-struct DevScratch {
-    void *p = nullptr;
-    ~DevScratch() { cudaFree(p); }
-};
-
 // the body of mksnap_gunzip_open; on failure the caller frees the state
 int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_len, const uint64_t *points,
             uint64_t n_points, mksnap_gunzip_info *info)
@@ -262,10 +247,10 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     // headers push the total past that is refused after the count (MKSNAP_E_CAPACITY)
     if (gz_len / 4 + 2 > 0xFFFFFFFFull)
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob of %llu bytes exceeds the 16 GiB limit", (unsigned long long)gz_len);
-    CK(h, cudaStreamCreateWithFlags(&g->s, cudaStreamNonBlocking));
+    CK(h, cudaStreamCreateWithFlags(g->s.put(), cudaStreamNonBlocking));
     const cudaStream_t s = g->s;
-    for (cudaEvent_t &e : g->ev)
-        CK(h, cudaEventCreate(&e));
+    for (Event &e : g->ev)
+        CK(h, cudaEventCreate(e.put()));
     mki::LinkState st;
     if (mki::link_start(&st, gz, gz_len) != mki::LINK_NEXT)
         return fail(h, MKSNAP_E_DATA, "gunzip: no gzip member header at offset 0");
@@ -273,7 +258,7 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     CK(h, cudaEventRecord(g->ev[5], h->s_comp));
     CK(h, cudaStreamWaitEvent(s, g->ev[5], 0));
     g->gz_len = gz_len;
-    CK(h, cudaMalloc(&g->d_gz, gz_len));
+    CK(h, g->d_gz.alloc(gz_len));
     CK(h, cudaMemcpyAsync(g->d_gz, gz, gz_len, cudaMemcpyHostToDevice, s));
     h->stats.h2d_bytes += gz_len;
 
@@ -283,12 +268,11 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     if (n_chunks > 0xFFFFFFF0ull)
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob too large");
     const uint64_t n_hchunks = (gz_len + gz::SCAN_CHUNK - 1) / gz::SCAN_CHUNK, body_words = gz_len / 32 + 1;
-    DevScratch cnt, body, tot; // tot: the 64-bit candidate total
-    CK(h, cudaMalloc(&cnt.p, (n_chunks + 1) * 4));
-    CK(h, cudaMalloc(&body.p, body_words * 4));
-    CK(h, cudaMalloc(&tot.p, 8));
-    uint32_t *const d_cnt = (uint32_t *)cnt.p, *const d_body = (uint32_t *)body.p;
-    unsigned long long *const d_tot = (unsigned long long *)tot.p;
+    DevBuf<uint32_t> d_cnt, d_body;
+    DevBuf<unsigned long long> d_tot; // the 64-bit candidate total
+    CK(h, d_cnt.alloc(n_chunks + 1));
+    CK(h, d_body.alloc(body_words));
+    CK(h, d_tot.alloc(1));
     CK(h, cudaMemsetAsync(d_cnt, 0, (n_chunks + 1) * 4, s));
     CK(h, cudaMemsetAsync(d_body, 0, body_words * 4, s));
     CK(h, cudaMemsetAsync(d_tot, 0, 8, s));
@@ -310,7 +294,7 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
             scan_words += n;
         }
     }
-    if (scan_words > h->scan_tmp_words)
+    if (scan_words > h->d_scan_tmp.size())
         return fail(h, MKSNAP_E_CAPACITY, "gunzip: blob too large for the scan scratch of this handle");
     int rc = scan_u32(h, d_cnt, d_cnt, n_chunks + 1, s);
     uint32_t total = 0;
@@ -321,7 +305,7 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
         g->n_cand = (uint64_t)total + 1;
         if (total64 != total || total64 + 2 > 0xFFFFFFFFull)
             rc = fail(h, MKSNAP_E_CAPACITY, "gunzip: %llu candidate starts exceed the 32-bit candidate scan", total64);
-        else if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess ||
+        else if (g->d_cand.alloc(g->n_cand) != cudaSuccess ||
                  cudaMemcpyAsync(g->d_cand, &st.pos, 8, cudaMemcpyHostToDevice, s) != cudaSuccess)
             rc = fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
         else if (n_chunks) {
@@ -335,35 +319,33 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     if (rc)
         return rc;
     CK(h, cudaGetLastError());
-    CK(h, cudaFree(body.p)); // the bitmap is not needed past the scan: keep it out of the count pass's peak
-    body.p = nullptr;
+    d_body.reset(); // the bitmap is not needed past the scan: keep it out of the count pass's peak
 
     // indexed open: the candidates become bit offsets, merged with the caller's points
     std::vector<uint64_t> byte_cand, bit_cand;
-    DevScratch rec, rec_n;
+    DevBuf<mki::Rec> rec;
+    DevBuf<unsigned long long> rec_n;
     mki::Recorder recorder{nullptr, nullptr, mki::REC_CAP};
     if (g->indexed) {
         byte_cand.resize(g->n_cand);
         CK(h, cudaMemcpyAsync(byte_cand.data(), g->d_cand, g->n_cand * 8, cudaMemcpyDeviceToHost, s));
         CK(h, cudaStreamSynchronize(s));
         bit_cand = mki::merge_points(byte_cand, points, n_points);
-        CK(h, cudaFree(g->d_cand));
-        g->d_cand = nullptr;
         g->n_cand = bit_cand.size();
-        if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess)
+        if (g->d_cand.alloc(g->n_cand) != cudaSuccess)
             return fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
         CK(h, cudaMemcpyAsync(g->d_cand, bit_cand.data(), g->n_cand * 8, cudaMemcpyHostToDevice, s));
-        CK(h, cudaMalloc(&rec.p, mki::REC_CAP * sizeof(mki::Rec)));
-        CK(h, cudaMalloc(&rec_n.p, 8));
-        CK(h, cudaMemsetAsync(rec_n.p, 0, 8, s));
-        recorder.buf = (mki::Rec *)rec.p;
-        recorder.n = (unsigned long long *)rec_n.p;
+        CK(h, rec.alloc(mki::REC_CAP));
+        CK(h, rec_n.alloc(1));
+        CK(h, cudaMemsetAsync(rec_n, 0, 8, s));
+        recorder.buf = rec;
+        recorder.n = rec_n;
         st.pos *= 8;
     }
     CK(h, cudaEventRecord(g->ev[1], s));
 
     // K5b count mode over every candidate
-    CK(h, cudaMalloc(&g->d_res, g->n_cand * sizeof(mki::SegRes)));
+    CK(h, g->d_res.alloc(g->n_cand));
     const uint64_t dgrid = (g->n_cand + gz::DEC_WARPS - 1) / gz::DEC_WARPS;
     if (g->indexed)
         gz::k_gz_decode_bits<<<(uint32_t)dgrid, 32 * gz::DEC_WARPS, 0, s>>>(
@@ -385,14 +367,13 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
     g->times.ms_count += gz_ms(g, 1, 2);
 
     // link: follow the true chain; starts without a usable count result are decoded again without the K limit
-    DevScratch one, one_res; // the start and result of such a decode
+    DevBuf<uint64_t> d_one; // the start and result of such a decode
+    DevBuf<mki::SegRes> d_one_res;
     const auto redecode = [&](uint64_t pos, mki::SegRes *r) -> int {
-        if (!one.p) {
-            CK(h, cudaMalloc(&one.p, 8));
-            CK(h, cudaMalloc(&one_res.p, sizeof(mki::SegRes)));
+        if (!d_one_res) {
+            CK(h, d_one.alloc(1));
+            CK(h, d_one_res.alloc(1));
         }
-        uint64_t *const d_one = (uint64_t *)one.p;
-        mki::SegRes *const d_one_res = (mki::SegRes *)one_res.p;
         CK(h, cudaMemcpyAsync(d_one, &pos, 8, cudaMemcpyHostToDevice, s));
         CK(h, cudaEventRecord(g->ev[1], s));
         if (g->indexed)
@@ -418,24 +399,21 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
                     (unsigned long long)(g->indexed ? st.pos / 8 : st.pos));
     if (lk != mki::LINK_DONE)
         return lk;
-    cudaFree(g->d_res);
-    g->d_res = nullptr;
+    g->d_res.reset(); // the count results are not needed past the link: keep them out of the windows' peak
     if (g->indexed) { // cut long segments at the records of their decode; the cuts join the write candidates
         unsigned long long n_rec = 0;
-        CK(h, cudaMemcpyAsync(&n_rec, rec_n.p, 8, cudaMemcpyDeviceToHost, s));
+        CK(h, cudaMemcpyAsync(&n_rec, rec_n, 8, cudaMemcpyDeviceToHost, s));
         CK(h, cudaStreamSynchronize(s));
         std::vector<mki::Rec> recs(std::min<uint64_t>(n_rec, mki::REC_CAP));
-        CK(h, cudaMemcpyAsync(recs.data(), rec.p, recs.size() * sizeof(mki::Rec), cudaMemcpyDeviceToHost, s));
+        CK(h, cudaMemcpyAsync(recs.data(), rec, recs.size() * sizeof(mki::Rec), cudaMemcpyDeviceToHost, s));
         CK(h, cudaStreamSynchronize(s));
         h->stats.d2h_bytes += recs.size() * sizeof(mki::Rec);
         const mki::IndexCounts c = mki::split_segments(&g->segs, std::move(recs), &cand, byte_cand, points, n_points,
                                                        &g->index);
         g->idx = mksnap_gunzip_index_info{n_points, c.linked, c.recorded, g->index.size()};
         if (c.recorded) {
-            CK(h, cudaFree(g->d_cand));
-            g->d_cand = nullptr;
             g->n_cand = cand.size();
-            if (cudaMalloc(&g->d_cand, g->n_cand * 8) != cudaSuccess)
+            if (g->d_cand.alloc(g->n_cand) != cudaSuccess)
                 return fail(h, MKSNAP_E_NOMEM, "gunzip: candidate table of %llu rows", (unsigned long long)g->n_cand);
             CK(h, cudaMemcpyAsync(g->d_cand, cand.data(), g->n_cand * 8, cudaMemcpyHostToDevice, s));
         }
@@ -458,20 +436,20 @@ int gz_open(mksnap *h, mksnap_gunzip_state *g, const uint8_t *gz, uint64_t gz_le
         k = w.seg1;
     }
     const uint64_t win_cap = std::max(gz::GZ_WINDOW, max_seg);
-    CK(h, cudaMalloc(&g->d_segs, g->segs.size() * sizeof(mki::Seg)));
+    CK(h, g->d_segs.alloc(g->segs.size()));
     CK(h, cudaMemcpyAsync(g->d_segs, g->segs.data(), g->segs.size() * sizeof(mki::Seg), cudaMemcpyHostToDevice, s));
-    CK(h, cudaMalloc(&g->d_seg_off, g->segs.size() * 8));
-    CK(h, cudaMalloc(&g->d_sym, win_cap * 2 + 64));
-    CK(h, cudaMalloc(&g->d_out, win_cap + 64)); // K0 reads up to 16 bytes past an extent
-    CK(h, cudaHostAlloc(&g->h_out, win_cap, cudaHostAllocDefault));
+    CK(h, g->d_seg_off.alloc(g->segs.size()));
+    CK(h, g->d_sym.alloc(win_cap + 32));
+    CK(h, g->d_out.alloc(win_cap + 64)); // K0 reads up to 16 bytes past an extent
+    CK(h, g->h_out.alloc(win_cap));
     for (int k = 0; k < 2; ++k)
-        CK(h, cudaMalloc(&g->d_hist[k], mki::WSIZE));
+        CK(h, g->d_hist[k].alloc(mki::WSIZE));
     CK(h, cudaMemsetAsync(g->d_hist[0], 0, mki::WSIZE, s));
-    g->ext_cap = 2 * max_mem_per_win;
-    CK(h, cudaMalloc(&g->d_ext, g->ext_cap * sizeof(CrcExtent)));
-    CK(h, cudaMalloc(&g->d_pb, (g->ext_cap + 1) * 4));
-    CK(h, cudaMalloc(&g->d_pure, (g->ext_cap + 1) * 4)); // the last word takes K0's stream accumulator
-    CK(h, cudaMalloc(&g->d_bad, 4));
+    const uint64_t ext_cap = 2 * max_mem_per_win;
+    CK(h, g->d_ext.alloc(ext_cap));
+    CK(h, g->d_pb.alloc(ext_cap + 1));
+    CK(h, g->d_pure.alloc(ext_cap + 1)); // the last word takes K0's stream accumulator
+    CK(h, g->d_bad.alloc(1));
     CK(h, cudaStreamSynchronize(s));
     g->mem_pure.assign(g->mems.size(), 0);
 
@@ -616,9 +594,6 @@ int gz_open_entry(mksnap_t *h, const void *gz, uint64_t gz_len, const uint64_t *
     CK(h, cudaSetDevice(h->cfg.device));
     memset(info, 0, sizeof *info);
     h->gz = new mksnap_gunzip_state();
-    memset(&h->gz->times, 0, sizeof h->gz->times);
-    for (cudaEvent_t &e : h->gz->ev)
-        e = nullptr;
     h->gz->indexed = indexed;
     const int rc = gz_open(h, h->gz, (const uint8_t *)gz, gz_len, points, n_points, info);
     if (rc) {
