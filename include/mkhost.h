@@ -301,6 +301,44 @@ int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost
                                           size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
                                           mkhost_gz_index_stats *stats, char *err, size_t errlen);
 
+/* Incremental layer ingest.  What a run of layers takes from a blob -- the member headers the merge reads, the DiffID,
+ * the tar length, the per-file SHA-256 values and the chunk digests of its files -- depends only on the blob's bytes
+ * and the CDC parameters, and the store files of base-image and cache-hit layers are content-addressed and almost
+ * never change between builds.  The layer cache remembers those values per caller key (makisu: the image store's file
+ * name, descriptor.Digest.Hex()), so an unchanged blob is REPLAYED: its remembered members go through the same merge
+ * (and, under MKHOST_FILE_DIGESTS, leave their remembered digests in the tree), its chunk digests join the session's
+ * table through mksnap_chunks_add and its DiffID comes from the record.  No byte of it is read, decompressed, uploaded
+ * or hashed; a replayed gzip layer also leaves its gz entry as it was.
+ * mkhost_memfs_update_from_tars_cached equals mkhost_memfs_update_from_tars_indexed(m, eng, gz, keys, ...) with the same
+ * arguments -- tree, remembered file digests, outs (DiffID, n_entries, tar_bytes per layer; root, n_chunks, n_unique of
+ * the run), refusals, and the state a failing layer leaves -- and with lc == NULL it is that call.  keys[i] == NULL:
+ * no cache for layer i.  An entry is replayed only when tar_fd is a regular file read from offset 0 whose device, inode,
+ * size, mtime and ctime (nanoseconds) are those it was recorded from, its MKHOST_GUNZIP flag is the recorded one, and
+ * it holds what the call needs (a DiffID unless MKHOST_NO_TAR_DIGEST, file digests under MKHOST_FILE_DIGESTS); under
+ * MKHOST_UNTAR nothing is replayed, since the files must be written.  Every other layer with a key and a regular file
+ * read from offset 0 is ingested as usual and recorded (replacing the entry under its key) once the whole run has
+ * finished; a call that fails records nothing.  A pipe is never replayed nor recorded.  The cache records the CDC
+ * parameters (mksnap_get_cdc); used with an engine cut under others it starts over.  One cache per image store, owned
+ * by the caller; save/load keep it between processes (a file that does not parse fails the load and leaves the cache
+ * as it was).  stats (may be NULL): layers of the call, of them replayed and recorded, bytes read from the layers' fds,
+ * chunk rows appended for replayed layers. */
+typedef struct mkhost_layer_cache mkhost_layer_cache;
+typedef struct {
+    uint64_t layers, layers_replayed, layers_recorded;
+    uint64_t blob_bytes_read; /* bytes read from the layers' fds by this call */
+    uint64_t chunks_appended; /* rows added through mksnap_chunks_add */
+} mkhost_layer_cache_stats;
+mkhost_layer_cache *mkhost_layer_cache_new(void);
+void mkhost_layer_cache_free(mkhost_layer_cache *c);
+uint64_t mkhost_layer_cache_size(const mkhost_layer_cache *c);
+int mkhost_layer_cache_save(const mkhost_layer_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_layer_cache_load(mkhost_layer_cache *c, const char *path, char *err, size_t errlen);
+int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_layer_cache *lc, mkhost_gz_index_cache *gz,
+                                         const char *const *keys, int64_t now_unix, const mkhost_tar_spec *layers,
+                                         size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
+                                         mkhost_layer_cache_stats *stats, mkhost_gz_index_stats *gz_stats, char *err,
+                                         size_t errlen);
+
 /* CopyOperation.Execute (lib/snapshot/copy_op.go:82-147) with fileio.Copier (lib/fileio/copy.go): what a COPY/ADD step
  * does to the file system when it runs with --modifyfs.  op->dst is used as the on-disk destination exactly like the
  * reference does (resolved against op->work_dir when relative).  mode selects the Copier of copy_op.go:98-124:

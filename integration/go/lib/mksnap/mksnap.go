@@ -448,3 +448,91 @@ func (fs *MemFS) UpdateFromTarsIndexed(e *Engine, gc *GzIndexCache, now int64, l
 	}
 	return res, nil
 }
+
+// LayerCache remembers what a run of layers took from each blob, per image-store digest (include/mkhost.h,
+// "Incremental layer ingest"): a later run replays an unchanged store file -- its remembered headers merged, its chunk
+// digests appended, its DiffID taken from the record -- instead of reading, decompressing and hashing it.  One cache
+// per image store, beside gz-index.cache; Save/Load keep it between makisu invocations.
+type LayerCache struct{ c *C.mkhost_layer_cache }
+
+// NewLayerCache loads `path` when it exists ("" = start cold).
+func NewLayerCache(path string) (*LayerCache, error) {
+	lc := &LayerCache{c: C.mkhost_layer_cache_new()}
+	runtime.SetFinalizer(lc, func(lc *LayerCache) { C.mkhost_layer_cache_free(lc.c) })
+	if path == "" {
+		return lc, nil
+	}
+	if _, err := os.Stat(path); err != nil {
+		return lc, nil
+	}
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_layer_cache_load(lc.c, cpath, errBuf, errLen) != 0 {
+		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return lc, nil
+}
+
+// Save writes the cache (next to the image store).
+func (lc *LayerCache) Save(path string) error {
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_layer_cache_save(lc.c, cpath, errBuf, errLen) != 0 {
+		return fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return nil
+}
+
+// UpdateFromTarsCached is UpdateFromTarsIndexed that replays every layer lc remembers under its Key for an unchanged
+// store file and records the others; lc == nil is UpdateFromTarsIndexed.  Results are those of the uncached run.
+func (fs *MemFS) UpdateFromTarsCached(e *Engine, lc *LayerCache, gc *GzIndexCache, now int64, layers []TarLayer, untar bool, flags uint32) ([]LayerResult, error) {
+	if untar {
+		flags |= 32 // MKHOST_UNTAR
+	}
+	n := len(layers)
+	if n == 0 {
+		return nil, nil
+	}
+	specs := make([]C.mkhost_tar_spec, n)
+	keys := make([]string, n)
+	for i, l := range layers {
+		specs[i].tar_fd = C.int(l.File.Fd())
+		specs[i].flags = C.uint32_t(l.Flags)
+		keys[i] = l.Key
+	}
+	ckeys, freeKeys := cStrings(keys)
+	defer freeKeys()
+	view := (*[1 << 28]*C.char)(unsafe.Pointer(ckeys))[:n:n]
+	for i := range keys {
+		if keys[i] == "" { // NULL key: no cache for this layer
+			C.free(unsafe.Pointer(view[i]))
+			view[i] = nil
+		}
+	}
+	var cache *C.mkhost_layer_cache
+	if lc != nil {
+		cache = lc.c
+	}
+	var gz *C.mkhost_gz_index_cache
+	if gc != nil {
+		gz = gc.c
+	}
+	outs := make([]C.mkhost_layer_result, n)
+	var st C.mkhost_layer_cache_stats
+	var gst C.mkhost_gz_index_stats
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	if rc := C.mkhost_memfs_update_from_tars_cached(fs.m, e.h, cache, gz, (**C.char)(unsafe.Pointer(ckeys)), C.int64_t(now),
+		&specs[0], C.size_t(n), C.uint32_t(flags), &outs[0], &st, &gst, errBuf, errLen); rc != 0 {
+		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	res := make([]LayerResult, n)
+	for i := range outs {
+		res[i] = toResult(&outs[i])
+	}
+	return res, nil
+}

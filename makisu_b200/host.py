@@ -40,6 +40,11 @@ class GzIndexStats(C.Structure):
                 ("points_linked", C.c_uint64), ("points_recorded", C.c_uint64)]
 
 
+class LayerCacheStats(C.Structure):
+    _fields_ = [("layers", C.c_uint64), ("layers_replayed", C.c_uint64), ("layers_recorded", C.c_uint64),
+                ("blob_bytes_read", C.c_uint64), ("chunks_appended", C.c_uint64)]
+
+
 class LayerSpec(C.Structure):
     _fields_ = [("ops", C.POINTER(CopyOp)), ("n_ops", C.c_size_t), ("tar_fd", C.c_int)]
 
@@ -119,6 +124,15 @@ SYMBOLS = [
                                                         C.POINTER(TarSpec), C.c_size_t, C.c_uint32,
                                                         C.POINTER(LayerResult), C.POINTER(GzIndexStats), C.c_char_p,
                                                         C.c_size_t]),
+    ("mkhost_layer_cache_new", _P, []),
+    ("mkhost_layer_cache_free", None, [_P]),
+    ("mkhost_layer_cache_size", C.c_uint64, [_P]),
+    ("mkhost_layer_cache_save", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_layer_cache_load", C.c_int, [_P, C.c_char_p, C.c_char_p, C.c_size_t]),
+    ("mkhost_memfs_update_from_tars_cached", C.c_int, [_P, _P, _P, _P, C.POINTER(C.c_char_p), C.c_int64,
+                                                       C.POINTER(TarSpec), C.c_size_t, C.c_uint32, C.POINTER(LayerResult),
+                                                       C.POINTER(LayerCacheStats), C.POINTER(GzIndexStats), C.c_char_p,
+                                                       C.c_size_t]),
     ("mkhost_copy_op_execute", C.c_int, [C.POINTER(CopyOp), C.c_uint32, C.POINTER(C.c_char_p), C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_eval_symlinks", C.c_size_t, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_cache_key", C.c_size_t, [C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]),
@@ -439,6 +453,23 @@ class MemFS:
             raise HostError(err.value.decode())
         return [_layer_dict(outs[i]) for i in range(n)], {k: getattr(st, k) for k, _ in GzIndexStats._fields_}
 
+    def update_from_tars_cached(self, eng: abi.Engine, cache: Optional["LayerCache"], gz: Optional["GzIndexCache"],
+                                keys: Sequence, now_unix: int, layers: Sequence, flags: int = 0):
+        """update_from_tars_indexed that replays the layers `cache` remembers under keys[i] for an unchanged store file,
+        and remembers the others.  -> (dicts, layer-cache stats dict, gz-index stats dict)."""
+        n = len(layers)
+        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
+        for i, l in enumerate(layers):
+            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
+        ks = (C.c_char_p * max(1, n))(*[k.encode() if k is not None else None for k in keys])
+        st, gst = LayerCacheStats(), GzIndexStats()
+        if load().mkhost_memfs_update_from_tars_cached(self.h, eng.h, cache.h if cache is not None else None,
+                                                       gz.h if gz is not None else None, ks, now_unix, specs, n, flags,
+                                                       outs, C.byref(st), C.byref(gst), err, len(err)):
+            raise HostError(err.value.decode())
+        return ([_layer_dict(outs[i]) for i in range(n)], {k: getattr(st, k) for k, _ in LayerCacheStats._fields_},
+                {k: getattr(gst, k) for k, _ in GzIndexStats._fields_})
+
     def commit_scan(self, eng: abi.Engine, now_unix: int, n_threads: int = 0, tar_fd: int = -1, flags: int = 0):
         err, out = C.create_string_buffer(1024), LayerResult()
         if load().mkhost_memfs_commit_scan(self.h, eng.h, now_unix, n_threads, tar_fd, flags, C.byref(out), err, len(err)):
@@ -589,6 +620,37 @@ class GzIndexCache:
     def close(self):
         if getattr(self, "h", None):
             load().mkhost_gz_index_cache_free(self.h)
+            self.h = None
+
+    __del__ = close
+
+
+class LayerCache:
+    """What a run of layers took from each blob, per image-store digest, remembered between builds: a later run replays
+    an unchanged store file instead of reading, decompressing and hashing it (include/mkhost.h, "Incremental layer
+    ingest"; MemFS.update_from_tars_cached)."""
+
+    def __init__(self, path: Optional[str] = None):
+        self.h = load().mkhost_layer_cache_new()
+        if path is not None and os.path.exists(path):
+            self.load(path)
+
+    def __len__(self):
+        return int(load().mkhost_layer_cache_size(self.h))
+
+    def load(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_layer_cache_load(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def save(self, path: str):
+        err = C.create_string_buffer(512)
+        if load().mkhost_layer_cache_save(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
+
+    def close(self):
+        if getattr(self, "h", None):
+            load().mkhost_layer_cache_free(self.h)
             self.h = None
 
     __del__ = close

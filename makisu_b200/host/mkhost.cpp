@@ -75,6 +75,11 @@ struct mkhost_chunk_cache {
     ChunkMemo memo;
 };
 
+// layer ingests per caller key, remembered between builds (incremental layer ingest, include/mkhost.h)
+struct mkhost_layer_cache {
+    LayerMemo memo;
+};
+
 // persistent snapshot.MemFS mirror (layers accumulate in the merged tree, like context.BuildContext.MemFS)
 struct mkhost_memfs {
     MemFS fs;
@@ -389,10 +394,12 @@ int update_from_tar_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int t
     }
 }
 
-// mkhost_memfs_update_from_tars; with `cache`, mkhost_memfs_update_from_tars_indexed (keys[i] for layer i)
+// mkhost_memfs_update_from_tars; with `cache`, mkhost_memfs_update_from_tars_indexed (keys[i] for layer i); with `lc`,
+// mkhost_memfs_update_from_tars_cached
 int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
                           size_t n_layers, uint32_t flags, mkhost_layer_result *outs, GzIndexMap *cache,
-                          const char *const *keys, mkhost_gz_index_stats *stats, char *err, size_t errlen)
+                          const char *const *keys, mkhost_gz_index_stats *stats, LayerMemo *lc,
+                          mkhost_layer_cache_stats *lstats, char *err, size_t errlen)
 {
     try {
         if (!m || !eng || (!layers && n_layers) || (!outs && n_layers))
@@ -416,18 +423,48 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
         // layer i's DiffID is stream slot i, deferred: the engine keeps its bytes in the stream log and hashes the
         // chains of the whole run together.  Per-file streams are inline, in the slots after the layers.
         const uint32_t file_base = (uint32_t)n_layers;
+        if (lc)
+            lc->bind(eng);
+        mkhost_layer_cache_stats lst{};
+        lst.layers = n_layers;
         ck(eng, mksnap_begin(eng), "begin");
         if (want_digest)
             ck(eng, mksnap_reserve_stream_log(eng, RUN_STREAM_LOG_BYTES), "reserve stream log");
         std::vector<uint64_t> entries(n_layers), tar_bytes(n_layers);
         std::vector<uint8_t> d;    // stream-digest rows [0, file_base + most file streams of a layer so far)
         uint32_t max_files = 0;
+        // layer cache: the DiffID of each replayed layer, the entry each recorded layer will leave (written after finish,
+        // when the DiffIDs exist), and where each layer's submitted bytes start in the session's chunk-end coordinates
+        std::vector<std::unique_ptr<std::array<uint8_t, 32>>> replayed(n_layers);
+        std::vector<std::unique_ptr<LayerMemo::Entry>> recording(n_layers);
+        std::vector<uint64_t> session_at(n_layers + 1, 0);
         for (size_t i = 0; i < n_layers; ++i) {
             // the layers join the tree (and the disk) strictly in order: whiteouts, overwrites and hard links of
             // layer i + 1 act on what layer i left
+            const uint32_t lflags = flags | layers[i].flags;
+            const char *key = keys ? keys[i] : nullptr;
+            FileId id;
+            const bool cacheable = lc && key && layer_file_id(layers[i].tar_fd, &id);
+            const LayerMemo::Entry *hit = cacheable && !(flags & MKHOST_UNTAR) ? lc->find(key, id, lflags) : nullptr;
+            session_at[i + 1] = session_at[i];
+            if (hit) { // replay: no read, no gunzip, no submit
+                IngestedLayer in;
+                in.members = hit->members;
+                const std::map<std::string, MemFile> layer = merge_layer(m->fs, flags, in, hit->file_digests.data(), 0);
+                const uint64_t n = hit->chunks.size() / 32;
+                for (uint64_t r0 = 0; r0 < n; r0 += MKSNAP_CHUNKS_ADD_MAX)
+                    ck(eng, mksnap_chunks_add(eng, hit->chunks.data() + 32 * r0, std::min<uint64_t>(MKSNAP_CHUNKS_ADD_MAX, n - r0)),
+                       "chunks add");
+                replayed[i].reset(new std::array<uint8_t, 32>(hit->diffid));
+                entries[i] = layer.size();
+                tar_bytes[i] = hit->tar_bytes;
+                lst.layers_replayed++;
+                lst.chunks_appended += n;
+                continue;
+            }
             IngestedLayer in;
-            const GzIndexUse ix{cache, keys ? keys[i] : nullptr, stats};
-            ingest_layer(m->fs, eng, layers[i].tar_fd, flags | layers[i].flags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in,
+            const GzIndexUse ix{cache, key, stats};
+            ingest_layer(m->fs, eng, layers[i].tar_fd, lflags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in,
                          cache && ix.key ? &ix : nullptr);
             if (in.n_file_streams) { // inline streams: their rows are final once the submits so far have run
                 max_files = std::max(max_files, in.n_file_streams);
@@ -437,20 +474,118 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
             const std::map<std::string, MemFile> layer = merge_layer(m->fs, flags, in, d.data(), file_base);
             entries[i] = layer.size();
             tar_bytes[i] = in.tar_bytes;
+            session_at[i + 1] += in.submitted;
+            lst.blob_bytes_read += in.blob_bytes;
+            if (cacheable) {
+                recording[i].reset(new LayerMemo::Entry);
+                LayerMemo::Entry &r = *recording[i];
+                r.id = id;
+                r.gunzip = (lflags & MKHOST_GUNZIP) != 0;
+                r.has_diffid = want_digest;
+                r.has_file_digests = file_digests;
+                r.tar_bytes = in.tar_bytes;
+                r.members = std::move(in.members);
+                if (in.n_file_streams) // rows file_base .. file_base + n_file_streams - 1 of d are this layer's files
+                    r.file_digests.assign(d.begin() + 32 * file_base, d.begin() + 32 * ((uint64_t)file_base + in.n_file_streams));
+            }
         }
         mksnap_result res;
         ck(eng, mksnap_finish(eng, &res), "finish");
         std::vector<uint8_t> rows(std::max<uint64_t>(res.n_streams, n_layers) * 32, 0);
         if (want_digest)
             ck(eng, mksnap_get_stream_digests(eng, rows.data(), rows.size() / 32), "stream digests");
-        for (size_t i = 0; i < n_layers; ++i) // root: chunk table of the whole run (one session)
+        for (size_t i = 0; i < n_layers; ++i) { // root: chunk table of the whole run (one session)
+            if (replayed[i])
+                memcpy(rows.data() + 32 * i, replayed[i]->data(), 32);
             set_layer_result(&outs[i], res, want_digest ? rows.data() + 32 * i : nullptr, entries[i], tar_bytes[i]);
+        }
+        if (std::any_of(recording.begin(), recording.end(), [](const auto &r) { return r != nullptr; })) {
+            // Every layer submitted arenas of its own, so the chunks it computed end inside its share of the session's
+            // bytes, (session_at[i], session_at[i + 1]]; rows appended for replayed layers carry end = UINT64_MAX.
+            std::vector<uint64_t> ends(std::max<uint64_t>(1, res.n_chunks));
+            std::vector<uint8_t> dig(32 * ends.size());
+            if (res.n_chunks)
+                ck(eng, mksnap_get_chunks(eng, ends.data(), dig.data(), res.n_chunks), "chunk table");
+            for (uint64_t c = 0; c < res.n_chunks; ++c) {
+                if (ends[c] == UINT64_MAX)
+                    continue;
+                if (ends[c] == 0 || ends[c] > session_at[n_layers])
+                    throw HostError("internal: the chunk table does not match the layers submitted");
+                const size_t i = std::upper_bound(session_at.begin(), session_at.end(), ends[c] - 1) - session_at.begin() - 1;
+                if (recording[i])
+                    recording[i]->chunks.insert(recording[i]->chunks.end(), dig.begin() + 32 * c, dig.begin() + 32 * (c + 1));
+            }
+            for (size_t i = 0; i < n_layers; ++i) {
+                if (!recording[i])
+                    continue;
+                if (want_digest)
+                    memcpy(recording[i]->diffid.data(), rows.data() + 32 * i, 32);
+                lc->e[keys[i]] = std::move(*recording[i]);
+                lst.layers_recorded++;
+            }
+        }
+        if (lstats)
+            *lstats = lst;
         return 0;
     } catch (const std::exception &e) {
         set_err(err, errlen, std::string("update memfs from tars: ") + e.what());
         return -1;
     }
 }
+
+const char LAYER_CACHE_MAGIC[] = "mkhost-layer-cache 1\n";
+
+struct LayerCacheWriter {
+    std::string b;
+    template <class T> void put(T v) { b.append((const char *)&v, sizeof v); }
+    void str(const std::string &s)
+    {
+        put<uint32_t>((uint32_t)s.size());
+        b += s;
+    }
+    void rows(const std::vector<uint8_t> &v)
+    {
+        put<uint64_t>(v.size() / 32);
+        if (!v.empty())
+            b.append((const char *)v.data(), v.size());
+    }
+};
+
+// every read is bounds-checked: a short or damaged file throws instead of reading past its end or allocating what
+// it cannot hold
+struct LayerCacheReader {
+    const uint8_t *p, *end;
+    template <class T> T get()
+    {
+        T v;
+        need(sizeof v);
+        memcpy(&v, p, sizeof v);
+        p += sizeof v;
+        return v;
+    }
+    void need(uint64_t n) const
+    {
+        if (n > (uint64_t)(end - p))
+            throw HostError("truncated");
+    }
+    std::string str()
+    {
+        const uint32_t n = get<uint32_t>();
+        need(n);
+        std::string s((const char *)p, n);
+        p += n;
+        return s;
+    }
+    std::vector<uint8_t> rows()
+    {
+        const uint64_t n = get<uint64_t>();
+        if (n > (uint64_t)(end - p) / 32)
+            throw HostError("truncated");
+        std::vector<uint8_t> v(p, p + 32 * n);
+        p += 32 * n;
+        return v;
+    }
+};
 
 } // namespace
 
@@ -465,7 +600,8 @@ int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
 int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
                                   size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
 {
-    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, nullptr, nullptr, nullptr, err, errlen);
+    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, nullptr, nullptr, nullptr, nullptr, nullptr,
+                                 err, errlen);
 }
 
 int mkhost_memfs_update_from_tar_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache, const char *key,
@@ -482,7 +618,136 @@ int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost
                                           mkhost_gz_index_stats *stats, char *err, size_t errlen)
 {
     return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, cache ? &cache->map : nullptr,
-                                 keys, stats, err, errlen);
+                                 keys, stats, nullptr, nullptr, err, errlen);
+}
+
+int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_layer_cache *lc, mkhost_gz_index_cache *gz,
+                                         const char *const *keys, int64_t now_unix, const mkhost_tar_spec *layers,
+                                         size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
+                                         mkhost_layer_cache_stats *stats, mkhost_gz_index_stats *gz_stats, char *err,
+                                         size_t errlen)
+{
+    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, gz ? &gz->map : nullptr, keys, gz_stats,
+                                 lc ? &lc->memo : nullptr, stats, err, errlen);
+}
+
+mkhost_layer_cache *mkhost_layer_cache_new(void) { return new mkhost_layer_cache; }
+void mkhost_layer_cache_free(mkhost_layer_cache *c) { delete c; }
+uint64_t mkhost_layer_cache_size(const mkhost_layer_cache *c) { return c ? c->memo.e.size() : 0; }
+
+// Binary, native byte order (little endian on the hosts this builds for): the line "mkhost-layer-cache 1\n", the CDC
+// parameters (5 x u32), the entry count (u64), then per entry: key (u32 length + bytes), file identity (dev, ino, size:
+// u64; mtime, ctime ns: i64), u8 bits (1 gunzip, 2 DiffID, 4 file digests), DiffID (32 bytes), tar_bytes (u64), members
+// (u64 count; each: name and linkname as u32 length + bytes, mode, uid, gid, size as i64, mtime ns as two u64 words,
+// low first, typeflag u8, data_len u64), file digests and chunk digests (u64 count + 32 bytes each).  Nothing follows.
+
+int mkhost_layer_cache_save(const mkhost_layer_cache *c, const char *path, char *err, size_t errlen)
+{
+    FILE *f = c && path ? fopen(path, "wb") : nullptr;
+    if (!f) {
+        set_err(err, errlen, std::string("save layer cache: ") + strerror(errno));
+        return -1;
+    }
+    LayerCacheWriter w;
+    w.b = LAYER_CACHE_MAGIC;
+    const mksnap_cdc_params &p = c->memo.cdc;
+    for (uint32_t v : {p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits})
+        w.put(v);
+    w.put<uint64_t>(c->memo.e.size());
+    for (const auto &kv : c->memo.e) {
+        const LayerMemo::Entry &x = kv.second;
+        w.str(kv.first);
+        w.put(x.id.dev), w.put(x.id.ino), w.put(x.id.size), w.put(x.id.mtime_ns), w.put(x.id.ctime_ns);
+        w.put<uint8_t>((x.gunzip ? 1 : 0) | (x.has_diffid ? 2 : 0) | (x.has_file_digests ? 4 : 0));
+        w.b.append((const char *)x.diffid.data(), 32);
+        w.put(x.tar_bytes);
+        w.put<uint64_t>(x.members.size());
+        for (const TarMember &m : x.members) {
+            const Hdr &h = m.hdr;
+            w.str(h.name), w.str(h.linkname);
+            w.put(h.mode), w.put(h.uid), w.put(h.gid), w.put(h.size);
+            w.put((uint64_t)(unsigned __int128)h.mtime_ns), w.put((uint64_t)((unsigned __int128)h.mtime_ns >> 64));
+            w.put<uint8_t>((uint8_t)h.typeflag);
+            w.put(m.data_len);
+        }
+        w.rows(x.file_digests);
+        w.rows(x.chunks);
+    }
+    const bool ok = fwrite(w.b.data(), 1, w.b.size(), f) == w.b.size() && !ferror(f);
+    const bool closed = fclose(f) == 0;
+    if (!ok || !closed)
+        set_err(err, errlen, std::string("save layer cache: ") + strerror(errno));
+    return ok && closed ? 0 : -1;
+}
+
+int mkhost_layer_cache_load(mkhost_layer_cache *c, const char *path, char *err, size_t errlen)
+{
+    if (!c || !path) {
+        set_err(err, errlen, "load layer cache: null argument");
+        return -1;
+    }
+    const int fd = open(path, O_RDONLY);
+    if (fd < 0) {
+        set_err(err, errlen, std::string("load layer cache: ") + strerror(errno));
+        return -1;
+    }
+    try {
+        std::vector<uint8_t> b;
+        try {
+            b = read_all(fd);
+        } catch (...) {
+            close(fd);
+            throw;
+        }
+        close(fd);
+        LayerCacheReader r{b.data(), b.data() + b.size()};
+        const size_t magic = sizeof LAYER_CACHE_MAGIC - 1;
+        r.need(magic);
+        if (memcmp(r.p, LAYER_CACHE_MAGIC, magic) != 0)
+            throw HostError("bad header");
+        r.p += magic;
+        LayerMemo memo;
+        mksnap_cdc_params &p = memo.cdc;
+        for (uint32_t *v : {&p.min_size, &p.normal_size, &p.max_size, &p.strict_bits, &p.loose_bits})
+            *v = r.get<uint32_t>();
+        const uint64_t n = r.get<uint64_t>();
+        for (uint64_t k = 0; k < n; ++k) {
+            const std::string key = r.str();
+            LayerMemo::Entry x;
+            x.id.dev = r.get<uint64_t>(), x.id.ino = r.get<uint64_t>(), x.id.size = r.get<uint64_t>();
+            x.id.mtime_ns = r.get<int64_t>(), x.id.ctime_ns = r.get<int64_t>();
+            const uint8_t bits = r.get<uint8_t>();
+            if (bits & ~7u)
+                throw HostError("bad entry");
+            x.gunzip = bits & 1, x.has_diffid = bits & 2, x.has_file_digests = bits & 4;
+            r.need(32);
+            memcpy(x.diffid.data(), r.p, 32);
+            r.p += 32;
+            x.tar_bytes = r.get<uint64_t>();
+            const uint64_t n_members = r.get<uint64_t>();
+            r.need(n_members / 64); // a member takes more than 64 bytes of the file
+            x.members.resize(n_members);
+            for (TarMember &m : x.members) {
+                Hdr &h = m.hdr;
+                h.name = r.str(), h.linkname = r.str();
+                h.mode = r.get<int64_t>(), h.uid = r.get<int64_t>(), h.gid = r.get<int64_t>(), h.size = r.get<int64_t>();
+                const uint64_t lo = r.get<uint64_t>(), hi = r.get<uint64_t>();
+                h.mtime_ns = (__int128)(((unsigned __int128)hi << 64) | lo);
+                h.typeflag = (char)r.get<uint8_t>();
+                m.data_len = r.get<uint64_t>();
+            }
+            x.file_digests = r.rows();
+            x.chunks = r.rows();
+            memo.e[key] = std::move(x);
+        }
+        if (r.p != r.end)
+            throw HostError("trailing bytes");
+        c->memo = std::move(memo);
+        return 0;
+    } catch (const std::exception &) {
+        set_err(err, errlen, "load layer cache: not a mkhost-layer-cache file");
+        return -1;
+    }
 }
 
 mkhost_gz_index_cache *mkhost_gz_index_cache_new(void) { return new mkhost_gz_index_cache; }
@@ -503,7 +768,8 @@ int mkhost_gz_index_cache_save(const mkhost_gz_index_cache *c, const char *path,
         if (kv.first.find('\n') != std::string::npos)
             continue;
         fprintf(f, "%llu %zu %s\n", (unsigned long long)kv.second.gz_len, kv.second.points.size(), kv.first.c_str());
-        fwrite(kv.second.points.data(), 8, kv.second.points.size(), f);
+        if (!kv.second.points.empty()) // an empty vector's data() may be null, which fwrite must not get
+            fwrite(kv.second.points.data(), 8, kv.second.points.size(), f);
     }
     const bool ok = !ferror(f) && fclose(f) == 0;
     if (!ok)
