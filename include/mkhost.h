@@ -77,7 +77,8 @@ int mkhost_context_crc32(mksnap_t *eng, const void *prefix, size_t prefix_len, c
  * unchanged file (tario.IsSimilarHeader: mtime to the second + size, lib/tario/compare.go:104-120).  Path strings,
  * link targets and the prefix are always streamed (tiny).  The result is bit-identical to mkhost_context_crc32 /
  * addCopyStep.SetCacheID whenever the remembered values are current; a cold cache degrades to the full computation and
- * fills itself.  The cache object belongs to the caller (one per build context); save/load keep it between processes. */
+ * fills itself.  The cache object belongs to the caller (one per build context); save/load keep it between processes (a
+ * file that does not parse fails the load and leaves the cache as it was; a loaded file merges into the cache). */
 typedef struct mkhost_crc_cache mkhost_crc_cache;
 typedef struct {
     uint64_t files_total, files_reused; /* regular files in the stream / folded from the cache */
@@ -182,8 +183,9 @@ int mkhost_memfs_commit_copy_ops(mkhost_memfs *m, mksnap_t *eng, int64_t now_uni
  * PCIe (mksnap_arena_submit_spans), and without tar_fd and MKHOST_MATERIALIZE it is not even read.  Every file chunked
  * by the commit is remembered.  The cache records the CDC parameters (mksnap_get_cdc); used with an engine cut under
  * others it starts over, nothing is an error.  One cache per build context, owned by the caller; save/load keep it
- * between processes.  stats: regular files of the layer and their bytes, files taken from the cache, bytes chunked on
- * the device, file bytes copied to the device. */
+ * between processes (a file that does not parse fails the load and leaves the cache as it was; a loaded file merges
+ * into the cache, or replaces it when it was saved under other CDC parameters).  stats: regular files of the layer and
+ * their bytes, files taken from the cache, bytes chunked on the device, file bytes copied to the device. */
 typedef struct mkhost_chunk_cache mkhost_chunk_cache;
 typedef struct {
     uint64_t files_total, files_reused;

@@ -528,31 +528,45 @@ def eval_symlinks(path: str, src_root: str) -> str:
     return os.fsdecode(buf.value)
 
 
-class CrcCache:
-    """pure(file content) per context file, remembered between builds: unchanged files are folded into the cacheID on
-    the host, only changed files travel to the device (include/mkhost.h, "Incremental cacheID")."""
+class _Cache:
+    """A libmkhost cache object (mkhost_<prefix>_cache_*), owned by the caller and kept between builds through its file:
+    a file that does not parse fails the load and leaves the cache as it was."""
+    _prefix = ""
 
     def __init__(self, path: Optional[str] = None):
-        self.h = load().mkhost_crc_cache_new()
+        self.h = self._fn("new")()
         if path is not None and os.path.exists(path):
-            err = C.create_string_buffer(512)
-            if load().mkhost_crc_cache_load(self.h, os.fsencode(path), err, len(err)):
-                raise HostError(err.value.decode())
+            self.load(path)
+
+    @classmethod
+    def _fn(cls, op: str):
+        return getattr(load(), "mkhost_%s_cache_%s" % (cls._prefix, op))
 
     def __len__(self):
-        return int(load().mkhost_crc_cache_size(self.h))
+        return int(self._fn("size")(self.h))
+
+    def load(self, path: str):
+        err = C.create_string_buffer(512)
+        if self._fn("load")(self.h, os.fsencode(path), err, len(err)):
+            raise HostError(err.value.decode())
 
     def save(self, path: str):
         err = C.create_string_buffer(512)
-        if load().mkhost_crc_cache_save(self.h, os.fsencode(path), err, len(err)):
+        if self._fn("save")(self.h, os.fsencode(path), err, len(err)):
             raise HostError(err.value.decode())
 
     def close(self):
         if getattr(self, "h", None):
-            load().mkhost_crc_cache_free(self.h)
+            self._fn("free")(self.h)
             self.h = None
 
     __del__ = close
+
+
+class CrcCache(_Cache):
+    """pure(file content) per context file, remembered between builds: unchanged files are folded into the cacheID on
+    the host, only changed files travel to the device (include/mkhost.h, "Incremental cacheID")."""
+    _prefix = "crc"
 
     def context_crc32(self, eng: abi.Engine, prefix: bytes, context_dir: str, from_paths: Sequence[str], n_threads: int = 0):
         """-> (crc32 as checksum.Sum32() returns it, stream length, stats dict)."""
@@ -565,92 +579,20 @@ class CrcCache:
         return crc.value, slen.value, {k: getattr(st, k) for k, _ in CrcCacheStats._fields_}
 
 
-class ChunkCache:
+class ChunkCache(_Cache):
     """Chunk digests per source file, remembered between builds: a layer commit takes an unchanged file's digests from
     here instead of chunking it again (include/mkhost.h, "Incremental layer commit"; MemFS.commit_copy_ops_cached)."""
-
-    def __init__(self, path: Optional[str] = None):
-        self.h = load().mkhost_chunk_cache_new()
-        if path is not None and os.path.exists(path):
-            self.load(path)
-
-    def __len__(self):
-        return int(load().mkhost_chunk_cache_size(self.h))
-
-    def load(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_chunk_cache_load(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def save(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_chunk_cache_save(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            load().mkhost_chunk_cache_free(self.h)
-            self.h = None
-
-    __del__ = close
+    _prefix = "chunk"
 
 
-class GzIndexCache:
+class GzIndexCache(_Cache):
     """Block indexes of single-member gzip layers, per image-store digest, remembered between builds: a later ingest
     of the same blob decodes it in parallel on the device (include/mkhost.h; MemFS.update_from_tar(s)_indexed)."""
-
-    def __init__(self, path: Optional[str] = None):
-        self.h = load().mkhost_gz_index_cache_new()
-        if path is not None and os.path.exists(path):
-            self.load(path)
-
-    def __len__(self):
-        return int(load().mkhost_gz_index_cache_size(self.h))
-
-    def load(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_gz_index_cache_load(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def save(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_gz_index_cache_save(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            load().mkhost_gz_index_cache_free(self.h)
-            self.h = None
-
-    __del__ = close
+    _prefix = "gz_index"
 
 
-class LayerCache:
+class LayerCache(_Cache):
     """What a run of layers took from each blob, per image-store digest, remembered between builds: a later run replays
     an unchanged store file instead of reading, decompressing and hashing it (include/mkhost.h, "Incremental layer
     ingest"; MemFS.update_from_tars_cached)."""
-
-    def __init__(self, path: Optional[str] = None):
-        self.h = load().mkhost_layer_cache_new()
-        if path is not None and os.path.exists(path):
-            self.load(path)
-
-    def __len__(self):
-        return int(load().mkhost_layer_cache_size(self.h))
-
-    def load(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_layer_cache_load(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def save(self, path: str):
-        err = C.create_string_buffer(512)
-        if load().mkhost_layer_cache_save(self.h, os.fsencode(path), err, len(err)):
-            raise HostError(err.value.decode())
-
-    def close(self):
-        if getattr(self, "h", None):
-            load().mkhost_layer_cache_free(self.h)
-            self.h = None
-
-    __del__ = close
+    _prefix = "layer"

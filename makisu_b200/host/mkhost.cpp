@@ -6,7 +6,7 @@
 //
 // One translation unit: the *.inc files in this directory are fragments of the anonymous namespace below, included in
 // dependency order (Go path helpers, Walk/Glob, context stream, file reader pool, tar writer, tar reader, Copier,
-// MemFS, arena packers); this file holds the C entry points.
+// MemFS, arena packers, cache files); this file holds the C entry points and the fields of each cache file.
 #include "../../include/mkhost.h"
 
 #include <dirent.h>
@@ -53,6 +53,7 @@ std::string errno_str(const std::string &what, const std::string &path)
 #include "copier.inc"
 #include "memfs.inc"
 #include "packer.inc"
+#include "cache_file.inc"
 
 } // namespace
 
@@ -63,21 +64,195 @@ struct mkhost_crc_cache {
         uint32_t pure;
     };
     std::map<std::string, Entry> files; // key: absolute path
+
+    // The file (cache_file.inc): "mkhost-crc-cache 1", then per file a line "<dev> <ino> <size> <mtime ns> <ctime ns>
+    // <pure as %08x> <path>", path last: it may hold spaces.
+    static constexpr const char *name = "crc", *kind = "crc";
+    void encode(CacheWriter &w) const
+    {
+        w.line("mkhost-crc-cache 1");
+        for (const auto &kv : files) {
+            char pure[16];
+            snprintf(pure, sizeof pure, " %08x", kv.second.pure);
+            w.entry(file_id_text(kv.second.id) + pure, kv.first);
+        }
+    }
+    void decode(CacheReader &r)
+    {
+        if (r.line() != "mkhost-crc-cache 1")
+            throw HostError("bad header");
+        while (!r.at_end()) {
+            const std::string s = r.line();
+            Entry x;
+            int used = 0, used2 = 0;
+            if (!parse_file_id(s.c_str(), &x.id, &used) || sscanf(s.c_str() + used, " %x %n", &x.pure, &used2) != 1 ||
+                used2 <= 0 || (size_t)(used + used2) >= s.size())
+                throw HostError("bad entry");
+            files[s.substr(used + used2)] = x;
+        }
+    }
+    void fold(mkhost_crc_cache &&f) // a loaded file merges into the cache
+    {
+        for (auto &kv : f.files)
+            files[kv.first] = kv.second;
+    }
 };
 
 // block indexes of gzip blobs per caller key, remembered between builds (include/mkhost.h)
 struct mkhost_gz_index_cache {
     GzIndexMap map;
+
+    // "mkhost-gz-index-cache 1", then per blob a line "<gz_len> <n_points> <key>" followed by its points, 8 bytes each
+    static constexpr const char *name = "gzip index", *kind = "gz-index";
+    void encode(CacheWriter &w) const
+    {
+        w.line("mkhost-gz-index-cache 1");
+        for (const auto &kv : map.e) {
+            const std::vector<uint64_t> &pts = kv.second.points;
+            if (w.entry(std::to_string(kv.second.gz_len) + " " + std::to_string(pts.size()), kv.first))
+                w.bytes(pts.data(), 8 * pts.size());
+        }
+    }
+    void decode(CacheReader &r)
+    {
+        if (r.line() != "mkhost-gz-index-cache 1")
+            throw HostError("bad header");
+        while (!r.at_end()) {
+            const std::string s = r.line();
+            unsigned long long len = 0, pts = 0;
+            int used = 0;
+            if (sscanf(s.c_str(), "%llu %llu %n", &len, &pts, &used) != 2 || used <= 0 || (size_t)used >= s.size())
+                throw HostError("bad entry");
+            map.e[s.substr(used)] = GzIndexMap::Entry{len, r.values<uint64_t>(pts)};
+        }
+    }
+    void fold(mkhost_gz_index_cache &&f) { map.e.swap(f.map.e); } // a loaded file replaces the cache
 };
 
 // chunk digests per source file, remembered between builds (incremental layer commit, include/mkhost.h)
 struct mkhost_chunk_cache {
     ChunkMemo memo;
+
+    // "mkhost-chunk-cache 1 <min> <normal> <max> <strict bits> <loose bits>", then per file a line
+    // "<dev> <ino> <size> <mtime ns> <ctime ns> <chunks> <path>" followed by its digests, 32 raw bytes per chunk
+    static constexpr const char *name = "chunk", *kind = "chunk";
+    void encode(CacheWriter &w) const
+    {
+        std::string h = "mkhost-chunk-cache 1";
+        const mksnap_cdc_params &p = memo.cdc;
+        for (uint32_t v : {p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits})
+            h += " " + std::to_string(v);
+        w.line(h);
+        for (const auto &kv : memo.files) {
+            const std::vector<uint8_t> &d = kv.second.digests;
+            if (w.entry(file_id_text(kv.second.id) + " " + std::to_string(d.size() / 32), kv.first))
+                w.bytes(d.data(), d.size());
+        }
+    }
+    void decode(CacheReader &r)
+    {
+        mksnap_cdc_params &p = memo.cdc;
+        const std::string h = r.line();
+        int used = 0;
+        if (sscanf(h.c_str(), "mkhost-chunk-cache 1 %u %u %u %u %u%n", &p.min_size, &p.normal_size, &p.max_size,
+                   &p.strict_bits, &p.loose_bits, &used) != 5 || (size_t)used != h.size())
+            throw HostError("bad header");
+        while (!r.at_end()) {
+            const std::string s = r.line();
+            ChunkMemo::Entry x;
+            unsigned long long rows = 0;
+            int used2 = 0;
+            if (!parse_file_id(s.c_str(), &x.id, &used) || sscanf(s.c_str() + used, " %llu %n", &rows, &used2) != 1 ||
+                used2 <= 0 || (size_t)(used + used2) >= s.size() || rows > x.id.size) // a chunk holds at least one byte
+                throw HostError("bad entry");
+            x.digests = r.rows(rows);
+            memo.files[s.substr(used + used2)] = std::move(x);
+        }
+    }
+    void fold(mkhost_chunk_cache &&f) // a loaded file merges into the cache, or replaces one cut under other parameters
+    {
+        if (memcmp(&f.memo.cdc, &memo.cdc, sizeof memo.cdc) != 0) {
+            memo.files.clear();
+            memo.cdc = f.memo.cdc; // a commit under other parameters starts over (ChunkMemo::bind)
+        }
+        for (auto &kv : f.memo.files)
+            memo.files[kv.first] = std::move(kv.second);
+    }
 };
 
 // layer ingests per caller key, remembered between builds (incremental layer ingest, include/mkhost.h)
 struct mkhost_layer_cache {
     LayerMemo memo;
+
+    // Binary: the line "mkhost-layer-cache 1", the CDC parameters (5 x u32), the entry count (u64), then per entry: key
+    // (u32 length + bytes), file identity (dev, ino, size: u64; mtime, ctime ns: i64), u8 bits (1 gunzip, 2 DiffID,
+    // 4 file digests), DiffID (32 bytes), tar_bytes (u64), members (u64 count; each: name and linkname as u32 length +
+    // bytes, mode, uid, gid, size as i64, mtime ns as two u64 words, low first, typeflag u8, data_len u64), file digests
+    // and chunk digests (u64 count + 32 bytes each).  Nothing follows.
+    static constexpr const char *name = "layer", *kind = "layer";
+    void encode(CacheWriter &w) const
+    {
+        w.line("mkhost-layer-cache 1");
+        const mksnap_cdc_params &p = memo.cdc;
+        for (uint32_t v : {p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits})
+            w.put(v);
+        w.put<uint64_t>(memo.e.size());
+        for (const auto &kv : memo.e) {
+            const LayerMemo::Entry &x = kv.second;
+            w.str(kv.first);
+            w.put(x.id.dev), w.put(x.id.ino), w.put(x.id.size), w.put(x.id.mtime_ns), w.put(x.id.ctime_ns);
+            w.put<uint8_t>((x.gunzip ? 1 : 0) | (x.has_diffid ? 2 : 0) | (x.has_file_digests ? 4 : 0));
+            w.bytes(x.diffid.data(), 32);
+            w.put(x.tar_bytes);
+            w.put<uint64_t>(x.members.size());
+            for (const TarMember &m : x.members) {
+                const Hdr &h = m.hdr;
+                w.str(h.name), w.str(h.linkname);
+                w.put(h.mode), w.put(h.uid), w.put(h.gid), w.put(h.size);
+                w.put((uint64_t)(unsigned __int128)h.mtime_ns), w.put((uint64_t)((unsigned __int128)h.mtime_ns >> 64));
+                w.put<uint8_t>((uint8_t)h.typeflag);
+                w.put(m.data_len);
+            }
+            w.rows(x.file_digests);
+            w.rows(x.chunks);
+        }
+    }
+    void decode(CacheReader &r)
+    {
+        if (r.line() != "mkhost-layer-cache 1")
+            throw HostError("bad header");
+        mksnap_cdc_params &p = memo.cdc;
+        for (uint32_t *v : {&p.min_size, &p.normal_size, &p.max_size, &p.strict_bits, &p.loose_bits})
+            *v = r.get<uint32_t>();
+        // nothing is sized by a count from the file: a count that lies runs out of file, entry by entry
+        for (uint64_t k = r.get<uint64_t>(); k > 0; --k) {
+            const std::string key = r.str();
+            LayerMemo::Entry x;
+            x.id.dev = r.get<uint64_t>(), x.id.ino = r.get<uint64_t>(), x.id.size = r.get<uint64_t>();
+            x.id.mtime_ns = r.get<int64_t>(), x.id.ctime_ns = r.get<int64_t>();
+            const uint8_t bits = r.get<uint8_t>();
+            if (bits & ~7u)
+                throw HostError("bad entry");
+            x.gunzip = bits & 1, x.has_diffid = bits & 2, x.has_file_digests = bits & 4;
+            memcpy(x.diffid.data(), r.take(32), 32);
+            x.tar_bytes = r.get<uint64_t>();
+            for (uint64_t n = r.get<uint64_t>(); n > 0; --n) {
+                TarMember m;
+                Hdr &h = m.hdr;
+                h.name = r.str(), h.linkname = r.str();
+                h.mode = r.get<int64_t>(), h.uid = r.get<int64_t>(), h.gid = r.get<int64_t>(), h.size = r.get<int64_t>();
+                const uint64_t lo = r.get<uint64_t>(), hi = r.get<uint64_t>();
+                h.mtime_ns = (__int128)(((unsigned __int128)hi << 64) | lo);
+                h.typeflag = (char)r.get<uint8_t>();
+                m.data_len = r.get<uint64_t>();
+                x.members.push_back(std::move(m));
+            }
+            x.file_digests = r.rows();
+            x.chunks = r.rows();
+            memo.e[key] = std::move(x);
+        }
+    }
+    void fold(mkhost_layer_cache &&f) { memo = std::move(f.memo); } // a loaded file replaces the cache
 };
 
 // persistent snapshot.MemFS mirror (layers accumulate in the merged tree, like context.BuildContext.MemFS)
@@ -533,60 +708,6 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
     }
 }
 
-const char LAYER_CACHE_MAGIC[] = "mkhost-layer-cache 1\n";
-
-struct LayerCacheWriter {
-    std::string b;
-    template <class T> void put(T v) { b.append((const char *)&v, sizeof v); }
-    void str(const std::string &s)
-    {
-        put<uint32_t>((uint32_t)s.size());
-        b += s;
-    }
-    void rows(const std::vector<uint8_t> &v)
-    {
-        put<uint64_t>(v.size() / 32);
-        if (!v.empty())
-            b.append((const char *)v.data(), v.size());
-    }
-};
-
-// every read is bounds-checked: a short or damaged file throws instead of reading past its end or allocating what
-// it cannot hold
-struct LayerCacheReader {
-    const uint8_t *p, *end;
-    template <class T> T get()
-    {
-        T v;
-        need(sizeof v);
-        memcpy(&v, p, sizeof v);
-        p += sizeof v;
-        return v;
-    }
-    void need(uint64_t n) const
-    {
-        if (n > (uint64_t)(end - p))
-            throw HostError("truncated");
-    }
-    std::string str()
-    {
-        const uint32_t n = get<uint32_t>();
-        need(n);
-        std::string s((const char *)p, n);
-        p += n;
-        return s;
-    }
-    std::vector<uint8_t> rows()
-    {
-        const uint64_t n = get<uint64_t>();
-        if (n > (uint64_t)(end - p) / 32)
-            throw HostError("truncated");
-        std::vector<uint8_t> v(p, p + 32 * n);
-        p += 32 * n;
-        return v;
-    }
-};
-
 } // namespace
 
 extern "C" {
@@ -635,183 +756,28 @@ mkhost_layer_cache *mkhost_layer_cache_new(void) { return new mkhost_layer_cache
 void mkhost_layer_cache_free(mkhost_layer_cache *c) { delete c; }
 uint64_t mkhost_layer_cache_size(const mkhost_layer_cache *c) { return c ? c->memo.e.size() : 0; }
 
-// Binary, native byte order (little endian on the hosts this builds for): the line "mkhost-layer-cache 1\n", the CDC
-// parameters (5 x u32), the entry count (u64), then per entry: key (u32 length + bytes), file identity (dev, ino, size:
-// u64; mtime, ctime ns: i64), u8 bits (1 gunzip, 2 DiffID, 4 file digests), DiffID (32 bytes), tar_bytes (u64), members
-// (u64 count; each: name and linkname as u32 length + bytes, mode, uid, gid, size as i64, mtime ns as two u64 words,
-// low first, typeflag u8, data_len u64), file digests and chunk digests (u64 count + 32 bytes each).  Nothing follows.
-
 int mkhost_layer_cache_save(const mkhost_layer_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "wb") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("save layer cache: ") + strerror(errno));
-        return -1;
-    }
-    LayerCacheWriter w;
-    w.b = LAYER_CACHE_MAGIC;
-    const mksnap_cdc_params &p = c->memo.cdc;
-    for (uint32_t v : {p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits})
-        w.put(v);
-    w.put<uint64_t>(c->memo.e.size());
-    for (const auto &kv : c->memo.e) {
-        const LayerMemo::Entry &x = kv.second;
-        w.str(kv.first);
-        w.put(x.id.dev), w.put(x.id.ino), w.put(x.id.size), w.put(x.id.mtime_ns), w.put(x.id.ctime_ns);
-        w.put<uint8_t>((x.gunzip ? 1 : 0) | (x.has_diffid ? 2 : 0) | (x.has_file_digests ? 4 : 0));
-        w.b.append((const char *)x.diffid.data(), 32);
-        w.put(x.tar_bytes);
-        w.put<uint64_t>(x.members.size());
-        for (const TarMember &m : x.members) {
-            const Hdr &h = m.hdr;
-            w.str(h.name), w.str(h.linkname);
-            w.put(h.mode), w.put(h.uid), w.put(h.gid), w.put(h.size);
-            w.put((uint64_t)(unsigned __int128)h.mtime_ns), w.put((uint64_t)((unsigned __int128)h.mtime_ns >> 64));
-            w.put<uint8_t>((uint8_t)h.typeflag);
-            w.put(m.data_len);
-        }
-        w.rows(x.file_digests);
-        w.rows(x.chunks);
-    }
-    const bool ok = fwrite(w.b.data(), 1, w.b.size(), f) == w.b.size() && !ferror(f);
-    const bool closed = fclose(f) == 0;
-    if (!ok || !closed)
-        set_err(err, errlen, std::string("save layer cache: ") + strerror(errno));
-    return ok && closed ? 0 : -1;
+    return save_cache(c, path, err, errlen);
 }
 
 int mkhost_layer_cache_load(mkhost_layer_cache *c, const char *path, char *err, size_t errlen)
 {
-    if (!c || !path) {
-        set_err(err, errlen, "load layer cache: null argument");
-        return -1;
-    }
-    const int fd = open(path, O_RDONLY);
-    if (fd < 0) {
-        set_err(err, errlen, std::string("load layer cache: ") + strerror(errno));
-        return -1;
-    }
-    try {
-        std::vector<uint8_t> b;
-        try {
-            b = read_all(fd);
-        } catch (...) {
-            close(fd);
-            throw;
-        }
-        close(fd);
-        LayerCacheReader r{b.data(), b.data() + b.size()};
-        const size_t magic = sizeof LAYER_CACHE_MAGIC - 1;
-        r.need(magic);
-        if (memcmp(r.p, LAYER_CACHE_MAGIC, magic) != 0)
-            throw HostError("bad header");
-        r.p += magic;
-        LayerMemo memo;
-        mksnap_cdc_params &p = memo.cdc;
-        for (uint32_t *v : {&p.min_size, &p.normal_size, &p.max_size, &p.strict_bits, &p.loose_bits})
-            *v = r.get<uint32_t>();
-        const uint64_t n = r.get<uint64_t>();
-        for (uint64_t k = 0; k < n; ++k) {
-            const std::string key = r.str();
-            LayerMemo::Entry x;
-            x.id.dev = r.get<uint64_t>(), x.id.ino = r.get<uint64_t>(), x.id.size = r.get<uint64_t>();
-            x.id.mtime_ns = r.get<int64_t>(), x.id.ctime_ns = r.get<int64_t>();
-            const uint8_t bits = r.get<uint8_t>();
-            if (bits & ~7u)
-                throw HostError("bad entry");
-            x.gunzip = bits & 1, x.has_diffid = bits & 2, x.has_file_digests = bits & 4;
-            r.need(32);
-            memcpy(x.diffid.data(), r.p, 32);
-            r.p += 32;
-            x.tar_bytes = r.get<uint64_t>();
-            const uint64_t n_members = r.get<uint64_t>();
-            r.need(n_members / 64); // a member takes more than 64 bytes of the file
-            x.members.resize(n_members);
-            for (TarMember &m : x.members) {
-                Hdr &h = m.hdr;
-                h.name = r.str(), h.linkname = r.str();
-                h.mode = r.get<int64_t>(), h.uid = r.get<int64_t>(), h.gid = r.get<int64_t>(), h.size = r.get<int64_t>();
-                const uint64_t lo = r.get<uint64_t>(), hi = r.get<uint64_t>();
-                h.mtime_ns = (__int128)(((unsigned __int128)hi << 64) | lo);
-                h.typeflag = (char)r.get<uint8_t>();
-                m.data_len = r.get<uint64_t>();
-            }
-            x.file_digests = r.rows();
-            x.chunks = r.rows();
-            memo.e[key] = std::move(x);
-        }
-        if (r.p != r.end)
-            throw HostError("trailing bytes");
-        c->memo = std::move(memo);
-        return 0;
-    } catch (const std::exception &) {
-        set_err(err, errlen, "load layer cache: not a mkhost-layer-cache file");
-        return -1;
-    }
+    return load_cache(c, path, err, errlen);
 }
 
 mkhost_gz_index_cache *mkhost_gz_index_cache_new(void) { return new mkhost_gz_index_cache; }
 void mkhost_gz_index_cache_free(mkhost_gz_index_cache *c) { delete c; }
 uint64_t mkhost_gz_index_cache_size(const mkhost_gz_index_cache *c) { return c ? c->map.e.size() : 0; }
 
-// "mkhost-gz-index-cache 1", then per blob a line "<gz_len> <n_points> <key>" followed by its points, 8 bytes each
-// (little endian)
 int mkhost_gz_index_cache_save(const mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "wb") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("save gzip index cache: ") + strerror(errno));
-        return -1;
-    }
-    fprintf(f, "mkhost-gz-index-cache 1\n");
-    for (const auto &kv : c->map.e) { // keys with newlines are not cached
-        if (kv.first.find('\n') != std::string::npos)
-            continue;
-        fprintf(f, "%llu %zu %s\n", (unsigned long long)kv.second.gz_len, kv.second.points.size(), kv.first.c_str());
-        if (!kv.second.points.empty()) // an empty vector's data() may be null, which fwrite must not get
-            fwrite(kv.second.points.data(), 8, kv.second.points.size(), f);
-    }
-    const bool ok = !ferror(f) && fclose(f) == 0;
-    if (!ok)
-        set_err(err, errlen, std::string("save gzip index cache: ") + strerror(errno));
-    return ok ? 0 : -1;
+    return save_cache(c, path, err, errlen);
 }
 
 int mkhost_gz_index_cache_load(mkhost_gz_index_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "rb") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("load gzip index cache: ") + strerror(errno));
-        return -1;
-    }
-    struct stat fst;
-    const uint64_t fsize = fstat(fileno(f), &fst) == 0 ? (uint64_t)fst.st_size : 0;
-    char *line = nullptr;
-    size_t cap = 0;
-    ssize_t n = getline(&line, &cap, f);
-    bool ok = n > 0 && strcmp(line, "mkhost-gz-index-cache 1\n") == 0;
-    std::map<std::string, GzIndexMap::Entry> e;
-    while (ok && (n = getline(&line, &cap, f)) > 0) {
-        if (line[n - 1] == '\n')
-            line[--n] = 0;
-        unsigned long long len = 0, pts = 0;
-        int used = 0;
-        if (sscanf(line, "%llu %llu %n", &len, &pts, &used) != 2 || used <= 0 || used >= n || pts > fsize / 8) {
-            ok = false; // the points must fit in what is left of the file
-            break;
-        }
-        GzIndexMap::Entry x{len, std::vector<uint64_t>(pts)};
-        ok = fread(x.points.data(), 8, pts, f) == pts;
-        e[line + used] = std::move(x);
-    }
-    free(line);
-    fclose(f);
-    if (!ok) {
-        set_err(err, errlen, "load gzip index cache: not a mkhost-gz-index-cache file");
-        return -1;
-    }
-    c->map.e.swap(e);
-    return 0;
+    return load_cache(c, path, err, errlen);
 }
 
 // ---- cache.Manager wire format (lib/cache/cache_manager.go:34-35,239-252) ----
@@ -1027,121 +993,26 @@ uint64_t mkhost_crc_cache_size(const mkhost_crc_cache *c) { return c ? c->files.
 
 int mkhost_crc_cache_save(const mkhost_crc_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "w") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("save crc cache: ") + strerror(errno));
-        return -1;
-    }
-    fprintf(f, "mkhost-crc-cache 1\n");
-    for (const auto &kv : c->files) // path last: it may hold spaces (newlines in file names are not cached)
-        if (kv.first.find('\n') == std::string::npos)
-            fprintf(f, "%s %08x %s\n", file_id_text(kv.second.id).c_str(), kv.second.pure, kv.first.c_str());
-    const bool ok = fclose(f) == 0;
-    if (!ok)
-        set_err(err, errlen, std::string("save crc cache: ") + strerror(errno));
-    return ok ? 0 : -1;
+    return save_cache(c, path, err, errlen);
 }
 
 int mkhost_crc_cache_load(mkhost_crc_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "r") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("load crc cache: ") + strerror(errno));
-        return -1;
-    }
-    char *line = nullptr;
-    size_t cap = 0;
-    ssize_t n = getline(&line, &cap, f);
-    bool ok = n > 0 && strncmp(line, "mkhost-crc-cache 1", 18) == 0;
-    while (ok && (n = getline(&line, &cap, f)) > 0) {
-        if (line[n - 1] == '\n')
-            line[--n] = 0;
-        FileId id;
-        unsigned pure;
-        int used = 0, used2 = 0;
-        if (!parse_file_id(line, &id, &used) || sscanf(line + used, " %x %n", &pure, &used2) != 1 || used2 <= 0 ||
-            used + used2 >= n) {
-            ok = false;
-            break;
-        }
-        c->files[line + used + used2] = mkhost_crc_cache::Entry{id, (uint32_t)pure};
-    }
-    free(line);
-    fclose(f);
-    if (!ok)
-        set_err(err, errlen, "load crc cache: not a mkhost-crc-cache file");
-    return ok ? 0 : -1;
+    return load_cache(c, path, err, errlen);
 }
 
 mkhost_chunk_cache *mkhost_chunk_cache_new(void) { return new mkhost_chunk_cache; }
 void mkhost_chunk_cache_free(mkhost_chunk_cache *c) { delete c; }
 uint64_t mkhost_chunk_cache_size(const mkhost_chunk_cache *c) { return c ? c->memo.files.size() : 0; }
 
-// "mkhost-chunk-cache 1 <min> <normal> <max> <strict bits> <loose bits>", then per file a line
-// "<dev> <ino> <size> <mtime ns> <ctime ns> <chunks> <path>" followed by its digests, 32 raw bytes per chunk
 int mkhost_chunk_cache_save(const mkhost_chunk_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "wb") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("save chunk cache: ") + strerror(errno));
-        return -1;
-    }
-    const mksnap_cdc_params &p = c->memo.cdc;
-    fprintf(f, "mkhost-chunk-cache 1 %u %u %u %u %u\n", p.min_size, p.normal_size, p.max_size, p.strict_bits, p.loose_bits);
-    for (const auto &kv : c->memo.files) { // newlines in file names are not cached
-        if (kv.first.find('\n') != std::string::npos)
-            continue;
-        fprintf(f, "%s %zu %s\n", file_id_text(kv.second.id).c_str(), kv.second.digests.size() / 32, kv.first.c_str());
-        fwrite(kv.second.digests.data(), 1, kv.second.digests.size(), f);
-    }
-    const bool ok = !ferror(f) && fclose(f) == 0;
-    if (!ok)
-        set_err(err, errlen, std::string("save chunk cache: ") + strerror(errno));
-    return ok ? 0 : -1;
+    return save_cache(c, path, err, errlen);
 }
 
 int mkhost_chunk_cache_load(mkhost_chunk_cache *c, const char *path, char *err, size_t errlen)
 {
-    FILE *f = c && path ? fopen(path, "rb") : nullptr;
-    if (!f) {
-        set_err(err, errlen, std::string("load chunk cache: ") + strerror(errno));
-        return -1;
-    }
-    char *line = nullptr;
-    size_t cap = 0;
-    mksnap_cdc_params p{};
-    ssize_t n = getline(&line, &cap, f);
-    bool ok = n > 0 && sscanf(line, "mkhost-chunk-cache 1 %u %u %u %u %u", &p.min_size, &p.normal_size, &p.max_size,
-                              &p.strict_bits, &p.loose_bits) == 5;
-    std::map<std::string, ChunkMemo::Entry> files;
-    while (ok && (n = getline(&line, &cap, f)) > 0) {
-        if (line[n - 1] == '\n')
-            line[--n] = 0;
-        ChunkMemo::Entry e;
-        unsigned long long rows = 0;
-        int used = 0, used2 = 0;
-        if (!parse_file_id(line, &e.id, &used) || sscanf(line + used, " %llu %n", &rows, &used2) != 1 || used2 <= 0 ||
-            used + used2 >= n || rows > (uint64_t)e.id.size) { // a chunk holds at least one byte
-            ok = false;
-            break;
-        }
-        e.digests.resize(32 * rows);
-        ok = fread(e.digests.data(), 1, e.digests.size(), f) == e.digests.size();
-        files[line + used + used2] = std::move(e);
-    }
-    free(line);
-    fclose(f);
-    if (!ok) {
-        set_err(err, errlen, "load chunk cache: not a mkhost-chunk-cache file");
-        return -1;
-    }
-    if (memcmp(&p, &c->memo.cdc, sizeof p) != 0) { // entries cut under other parameters do not mix with these
-        c->memo.files.clear();
-        c->memo.cdc = p; // a commit under other parameters starts over (ChunkMemo::bind)
-    }
-    for (auto &kv : files)
-        c->memo.files[kv.first] = std::move(kv.second);
-    return 0;
+    return load_cache(c, path, err, errlen);
 }
 
 int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const void *prefix, size_t prefix_len,

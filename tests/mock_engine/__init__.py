@@ -47,6 +47,22 @@ def _build(sanitize: bool) -> str:
     return so
 
 
+SANITIZED_HOST = "MKHOST_TEST_SANITIZED_LIB"  # load_for_child loads libmkhost from here instead of the package
+
+
+@functools.cache
+def sanitized_host() -> str:
+    """Path of libmkhost built with ASan/UBSan, once per process, outside the tree: set SANITIZED_HOST to it in the
+    environment of run(..., sanitize=True)."""
+    so = os.path.join(_out_dir(), "libmkhost_asan.so")
+    lib = os.path.join(ROOT, "makisu_b200", "lib")
+    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-pthread",
+                           "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer",
+                           "-I", os.path.join(ROOT, "include"), "-o", so, os.path.join(ROOT, "makisu_b200", "host", "mkhost.cpp"),
+                           "-L", lib, "-lmksnap", "-Wl,-rpath," + lib, "-ldl"])
+    return so
+
+
 def run(module: str, scenario: str, tmp, sanitize: bool = False) -> subprocess.CompletedProcess:
     """python -m <module> <mock.so> <scenario> <tmp> in a fresh process; it must exit 0 with no sanitizer report."""
     env = dict(os.environ)
@@ -67,6 +83,9 @@ def load_for_child(path: str, host: bool = False) -> C.CDLL:
     mock = C.CDLL(path, mode=C.RTLD_GLOBAL)  # BEFORE anything loads libmksnap / libmkhost
     if host:
         from makisu_b200 import host as mkhost
+        if os.environ.get(SANITIZED_HOST):
+            from pathlib import Path
+            mkhost.LIB_PATH = Path(os.environ[SANITIZED_HOST])
         mkhost.load()
         seen = C.CDLL(None)
         for name in ENTRY_POINTS:

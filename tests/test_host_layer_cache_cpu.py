@@ -7,19 +7,13 @@ AddressSanitizer and UndefinedBehaviorSanitizer.  Each runs in a fresh process t
 before libmkhost:
     python -m tests.test_host_layer_cache_cpu <mock.so> <scenario> <tmpdir>"""
 import ctypes as C
-import functools
 import os
-import subprocess
 import sys
-import tempfile
 
 import pytest
 
 from tests import layer_cache_cases as cases
 from tests import mock_engine
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-SANITIZED_HOST = "MKHOST_TEST_SANITIZED_LIB"  # the child loads libmkhost from here instead of the package
 
 
 @pytest.mark.parametrize("scenario", cases.ALL + ["untar"])
@@ -30,20 +24,8 @@ def test_layer_cache_mock(tmp_path, scenario):
     assert scenario + " ok" in r.stdout
 
 
-@functools.cache
-def _sanitized_host() -> str:
-    d = tempfile.mkdtemp(prefix="mkhost_asan_")
-    so = os.path.join(d, "libmkhost.so")
-    lib = os.path.join(ROOT, "makisu_b200", "lib")
-    subprocess.check_call(["g++", "-O1", "-g", "-std=c++17", "-fPIC", "-shared", "-pthread",
-                           "-fsanitize=address,undefined", "-fno-sanitize-recover=all", "-fno-omit-frame-pointer",
-                           "-I", os.path.join(ROOT, "include"), "-o", so, os.path.join(ROOT, "makisu_b200", "host", "mkhost.cpp"),
-                           "-L", lib, "-lmksnap", "-Wl,-rpath," + lib, "-ldl"])
-    return so
-
-
 def test_layer_cache_under_asan_ubsan(tmp_path, monkeypatch):
-    monkeypatch.setenv(SANITIZED_HOST, _sanitized_host())
+    monkeypatch.setenv(mock_engine.SANITIZED_HOST, mock_engine.sanitized_host())
     r = mock_engine.run("tests.test_host_layer_cache_cpu", "every", tmp_path, sanitize=True)
     assert "every ok" in r.stdout
 
@@ -72,11 +54,6 @@ def every(make, tmp):
 
 def main():
     mock_path, scenario, tmp = sys.argv[1:4]
-    if os.environ.get(SANITIZED_HOST):
-        from pathlib import Path
-
-        from makisu_b200 import host
-        host.LIB_PATH = Path(os.environ[SANITIZED_HOST])
     mock = mock_engine.load_for_child(mock_path, host=True)
 
     def make(arena, **kw):
