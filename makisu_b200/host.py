@@ -326,6 +326,19 @@ def _layer_dict(out: LayerResult):
             "tar_bytes": out.tar_bytes, "n_chunks": out.n_chunks, "n_unique": out.n_unique}
 
 
+def _run_layers(layers: Sequence, keys: Sequence, call) -> List[dict]:
+    """A run of layers through a C entry point: layers[i] is tar_fd or (tar_fd, per-layer flags such as MKHOST_GUNZIP),
+    keys[i] a str or None.  call(specs, n, keys, outs, err) makes the C call.  -> one result dict per layer."""
+    n = len(layers)
+    specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
+    for i, l in enumerate(layers):
+        specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
+    ks = (C.c_char_p * max(1, n))(*[k.encode() if k is not None else None for k in keys])
+    if call(specs, n, ks, outs, err):
+        raise HostError(err.value.decode())
+    return [_layer_dict(outs[i]) for i in range(n)]
+
+
 class MemFS:
     """snapshot.NewMemFS(clk, root, blacklist): layers accumulate; AddLayerByCopyOps / AddLayerByScan either
     described as text (no GPU) or committed through an Engine."""
@@ -420,13 +433,8 @@ class MemFS:
         """A run of layers applied in order in ONE engine session, their DiffID chains hashed together.  layers: tar_fd
         or (tar_fd, per-layer flags such as MKHOST_GUNZIP) per layer.  -> one dict per layer, as update_from_tar gives;
         root / n_chunks / n_unique are those of the whole run."""
-        n = len(layers)
-        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
-        for i, l in enumerate(layers):
-            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
-        if load().mkhost_memfs_update_from_tars(self.h, eng.h, now_unix, specs, n, flags, outs, err, len(err)):
-            raise HostError(err.value.decode())
-        return [_layer_dict(outs[i]) for i in range(n)]
+        return _run_layers(layers, (), lambda specs, n, ks, outs, err: load().mkhost_memfs_update_from_tars(
+            self.h, eng.h, now_unix, specs, n, flags, outs, err, len(err)))
 
     def update_from_tar_indexed(self, eng: abi.Engine, cache: Optional["GzIndexCache"], key: Optional[str],
                                 now_unix: int, tar_fd: int, flags: int = 0):
@@ -442,32 +450,21 @@ class MemFS:
     def update_from_tars_indexed(self, eng: abi.Engine, cache: Optional["GzIndexCache"], keys: Sequence,
                                  now_unix: int, layers: Sequence, flags: int = 0):
         """update_from_tars with a block-index cache: keys[i] (or None) for layer i.  -> (dicts, stats dict)."""
-        n = len(layers)
-        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
-        for i, l in enumerate(layers):
-            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
-        ks = (C.c_char_p * max(1, n))(*[k.encode() if k is not None else None for k in keys])
         st = GzIndexStats()
-        if load().mkhost_memfs_update_from_tars_indexed(self.h, eng.h, cache.h if cache is not None else None, ks, now_unix, specs,
-                                                        n, flags, outs, C.byref(st), err, len(err)):
-            raise HostError(err.value.decode())
-        return [_layer_dict(outs[i]) for i in range(n)], {k: getattr(st, k) for k, _ in GzIndexStats._fields_}
+        res = _run_layers(layers, keys, lambda specs, n, ks, outs, err: load().mkhost_memfs_update_from_tars_indexed(
+            self.h, eng.h, cache.h if cache is not None else None, ks, now_unix, specs, n, flags, outs, C.byref(st), err,
+            len(err)))
+        return res, {k: getattr(st, k) for k, _ in GzIndexStats._fields_}
 
     def update_from_tars_cached(self, eng: abi.Engine, cache: Optional["LayerCache"], gz: Optional["GzIndexCache"],
                                 keys: Sequence, now_unix: int, layers: Sequence, flags: int = 0):
         """update_from_tars_indexed that replays the layers `cache` remembers under keys[i] for an unchanged store file,
         and remembers the others.  -> (dicts, layer-cache stats dict, gz-index stats dict)."""
-        n = len(layers)
-        specs, outs, err = (TarSpec * max(1, n))(), (LayerResult * max(1, n))(), C.create_string_buffer(1024)
-        for i, l in enumerate(layers):
-            specs[i].tar_fd, specs[i].flags = (l, 0) if isinstance(l, int) else l
-        ks = (C.c_char_p * max(1, n))(*[k.encode() if k is not None else None for k in keys])
         st, gst = LayerCacheStats(), GzIndexStats()
-        if load().mkhost_memfs_update_from_tars_cached(self.h, eng.h, cache.h if cache is not None else None,
-                                                       gz.h if gz is not None else None, ks, now_unix, specs, n, flags,
-                                                       outs, C.byref(st), C.byref(gst), err, len(err)):
-            raise HostError(err.value.decode())
-        return ([_layer_dict(outs[i]) for i in range(n)], {k: getattr(st, k) for k, _ in LayerCacheStats._fields_},
+        res = _run_layers(layers, keys, lambda specs, n, ks, outs, err: load().mkhost_memfs_update_from_tars_cached(
+            self.h, eng.h, cache.h if cache is not None else None, gz.h if gz is not None else None, ks, now_unix, specs, n,
+            flags, outs, C.byref(st), C.byref(gst), err, len(err)))
+        return (res, {k: getattr(st, k) for k, _ in LayerCacheStats._fields_},
                 {k: getattr(gst, k) for k, _ in GzIndexStats._fields_})
 
     def commit_scan(self, eng: abi.Engine, now_unix: int, n_threads: int = 0, tar_fd: int = -1, flags: int = 0):

@@ -26,6 +26,7 @@
 #include <map>
 #include <memory>
 #include <mutex>
+#include <optional>
 #include <stdexcept>
 #include <chrono>
 #include <string>
@@ -545,36 +546,13 @@ size_t mkhost_memfs_describe_update_from_tar(mkhost_memfs *m, int64_t now_unix, 
 
 namespace {
 
-// mkhost_memfs_update_from_tar; with `ix`, mkhost_memfs_update_from_tar_indexed
-int update_from_tar_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
-                         mkhost_layer_result *out, const GzIndexUse *ix, char *err, size_t errlen)
-{
-    try {
-        m->fs.set_now(now_unix);
-        const bool want_digest = !(flags & MKHOST_NO_TAR_DIGEST);
-        ck(eng, mksnap_begin(eng), "begin");
-        IngestedLayer in;
-        ingest_layer(m->fs, eng, tar_fd, flags, 0, 0, 1, in, ix);
-        mksnap_result res;
-        ck(eng, mksnap_finish(eng, &res), "finish");
-        std::vector<uint8_t> d((in.n_file_streams + 1) * 32, 0);
-        if (want_digest || in.n_file_streams)
-            ck(eng, mksnap_get_stream_digests(eng, d.data(), in.n_file_streams + 1), "stream digests");
-        const std::map<std::string, MemFile> layer = merge_layer(m->fs, flags, in, d.data(), 1);
-        set_layer_result(out, res, want_digest ? d.data() : nullptr, layer.size(), in.tar_bytes);
-        return 0;
-    } catch (const std::exception &e) {
-        set_err(err, errlen, std::string("update memfs from tar: ") + e.what());
-        return -1;
-    }
-}
-
 // mkhost_memfs_update_from_tars; with `cache`, mkhost_memfs_update_from_tars_indexed (keys[i] for layer i); with `lc`,
-// mkhost_memfs_update_from_tars_cached
+// mkhost_memfs_update_from_tars_cached.  tar_flags: the range flags of the layers' tar streams (MKSNAP_R_DEFER for a
+// run, which then reserves the stream log; 0 for a single layer, whose one stream stays inline).  `what` prefixes errors.
 int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
-                          size_t n_layers, uint32_t flags, mkhost_layer_result *outs, GzIndexMap *cache,
+                          size_t n_layers, uint32_t flags, uint32_t tar_flags, mkhost_layer_result *outs, GzIndexMap *cache,
                           const char *const *keys, mkhost_gz_index_stats *stats, LayerMemo *lc,
-                          mkhost_layer_cache_stats *lstats, char *err, size_t errlen)
+                          mkhost_layer_cache_stats *lstats, const char *what, char *err, size_t errlen)
 {
     try {
         if (!m || !eng || (!layers && n_layers) || (!outs && n_layers))
@@ -595,15 +573,15 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
             throw HostError("a run of " + std::to_string(n_layers) + " layers needs a stream slot per layer" +
                             (file_digests ? " and more for the per-file digests" : "") + ": engine max_extents (" +
                             std::to_string(lim.max_streams) + ") is too small");
-        // layer i's DiffID is stream slot i, deferred: the engine keeps its bytes in the stream log and hashes the
-        // chains of the whole run together.  Per-file streams are inline, in the slots after the layers.
+        // layer i's DiffID is stream slot i; under MKSNAP_R_DEFER the engine keeps its bytes in the stream log and hashes
+        // the chains of the whole run together.  Per-file streams are inline, in the slots after the layers.
         const uint32_t file_base = (uint32_t)n_layers;
         if (lc)
             lc->bind(eng);
         mkhost_layer_cache_stats lst{};
         lst.layers = n_layers;
         ck(eng, mksnap_begin(eng), "begin");
-        if (want_digest)
+        if (want_digest && (tar_flags & MKSNAP_R_DEFER))
             ck(eng, mksnap_reserve_stream_log(eng, RUN_STREAM_LOG_BYTES), "reserve stream log");
         std::vector<uint64_t> entries(n_layers), tar_bytes(n_layers);
         std::vector<uint8_t> d;    // stream-digest rows [0, file_base + most file streams of a layer so far)
@@ -639,7 +617,7 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
             }
             IngestedLayer in;
             const GzIndexUse ix{cache, key, stats};
-            ingest_layer(m->fs, eng, layers[i].tar_fd, lflags, (uint32_t)i, MKSNAP_R_DEFER, file_base, in,
+            ingest_layer(m->fs, eng, layers[i].tar_fd, lflags, (uint32_t)i, tar_flags, file_base, in,
                          cache && ix.key ? &ix : nullptr);
             if (in.n_file_streams) { // inline streams: their rows are final once the submits so far have run
                 max_files = std::max(max_files, in.n_file_streams);
@@ -703,7 +681,7 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
             *lstats = lst;
         return 0;
     } catch (const std::exception &e) {
-        set_err(err, errlen, std::string("update memfs from tars: ") + e.what());
+        set_err(err, errlen, what + std::string(e.what()));
         return -1;
     }
 }
@@ -715,22 +693,25 @@ extern "C" {
 int mkhost_memfs_update_from_tar(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, int tar_fd, uint32_t flags,
                                  mkhost_layer_result *out, char *err, size_t errlen)
 {
-    return update_from_tar_impl(m, eng, now_unix, tar_fd, flags, out, nullptr, err, errlen);
+    return mkhost_memfs_update_from_tar_indexed(m, eng, nullptr, nullptr, now_unix, tar_fd, flags, out, nullptr, err, errlen);
 }
 
 int mkhost_memfs_update_from_tars(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_tar_spec *layers,
                                   size_t n_layers, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
 {
-    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, nullptr, nullptr, nullptr, nullptr, nullptr,
-                                 err, errlen);
+    return mkhost_memfs_update_from_tars_cached(m, eng, nullptr, nullptr, nullptr, now_unix, layers, n_layers, flags, outs,
+                                                nullptr, nullptr, err, errlen);
 }
 
+// a single layer is a run of one whose DiffID stream stays inline; flag bits the run does not take are ignored
 int mkhost_memfs_update_from_tar_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache, const char *key,
                                          int64_t now_unix, int tar_fd, uint32_t flags, mkhost_layer_result *out,
                                          mkhost_gz_index_stats *stats, char *err, size_t errlen)
 {
-    const GzIndexUse ix{cache ? &cache->map : nullptr, key, stats};
-    return update_from_tar_impl(m, eng, now_unix, tar_fd, flags, out, cache && key ? &ix : nullptr, err, errlen);
+    const mkhost_tar_spec layer{tar_fd, flags & MKHOST_GUNZIP};
+    return update_from_tars_impl(m, eng, now_unix, &layer, 1, flags & (MKHOST_NO_TAR_DIGEST | MKHOST_FILE_DIGESTS | MKHOST_UNTAR),
+                                 0, out, cache ? &cache->map : nullptr, &key, stats, nullptr, nullptr,
+                                 "update memfs from tar: ", err, errlen);
 }
 
 int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost_gz_index_cache *cache,
@@ -738,8 +719,8 @@ int mkhost_memfs_update_from_tars_indexed(mkhost_memfs *m, mksnap_t *eng, mkhost
                                           size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
                                           mkhost_gz_index_stats *stats, char *err, size_t errlen)
 {
-    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, cache ? &cache->map : nullptr,
-                                 keys, stats, nullptr, nullptr, err, errlen);
+    return mkhost_memfs_update_from_tars_cached(m, eng, nullptr, cache, keys, now_unix, layers, n_layers, flags, outs, nullptr,
+                                                stats, err, errlen);
 }
 
 int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_layer_cache *lc, mkhost_gz_index_cache *gz,
@@ -748,8 +729,8 @@ int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_
                                          mkhost_layer_cache_stats *stats, mkhost_gz_index_stats *gz_stats, char *err,
                                          size_t errlen)
 {
-    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, outs, gz ? &gz->map : nullptr, keys, gz_stats,
-                                 lc ? &lc->memo : nullptr, stats, err, errlen);
+    return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, MKSNAP_R_DEFER, outs, gz ? &gz->map : nullptr,
+                                 keys, gz_stats, lc ? &lc->memo : nullptr, stats, "update memfs from tars: ", err, errlen);
 }
 
 mkhost_layer_cache *mkhost_layer_cache_new(void) { return new mkhost_layer_cache; }
@@ -845,131 +826,177 @@ int mkhost_cache_chunk_entry_parse(const char *entry, uint8_t root[32], uint64_t
     return 0;
 }
 
+} // extern "C"
+
+namespace {
+
+double ms_since(std::chrono::steady_clock::time_point t)
+{
+    return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
+}
+
+using FileKey = std::tuple<std::string, uint64_t, uint64_t, uint64_t, int64_t, int64_t>; // path, dev, ino, size, mtime, ctime
+FileKey file_key(const Seg &g) { return FileKey{g.path, g.id.dev, g.id.ino, g.size, g.id.mtime_ns, g.id.ctime_ns}; }
+
+// One engine session of a cacheID pass as CRC extents, numbered as mksnap_get_extent_crcs returns them: path strings at
+// 16-byte alignment, file contents at 512-byte alignment with 4 KiB of room.  CRC is linear, so a file is split across
+// arenas at any 16-byte boundary; remember() joins its pieces again after finish.
+struct CrcPacker {
+    struct Sent { // a file that travelled: its extents [first, first + n)
+        const Seg *seg;
+        uint64_t first, n;
+    };
+    ArenaSession s;
+    std::vector<uint64_t> len; // length of every CRC extent so far, by extent index
+    std::vector<Sent> sent;
+    double ms_reads = 0, ms_acquire = 0, ms_submit = 0; // reading files, waiting for an arena, submitting it
+    std::chrono::steady_clock::time_point t;
+
+    // begins the session and leases its first arena
+    CrcPacker(mksnap_t *eng, int n_threads) : s(eng, n_threads, 1) // cap unrounded: CRC pieces end anywhere
+    {
+        s.after_reads = [this]() {
+            ms_reads += ms_since(t);
+            t = std::chrono::steady_clock::now();
+        };
+        ck(eng, mksnap_begin(eng), "begin");
+        acquire();
+    }
+    void acquire()
+    {
+        t = std::chrono::steady_clock::now();
+        s.acquire();
+        ms_acquire += ms_since(t);
+    }
+    void submit()
+    {
+        t = std::chrono::steady_clock::now();
+        s.submit();
+        ms_submit += ms_since(t);
+    }
+    void finish(mksnap_result &res) { ck(s.eng, mksnap_finish(s.eng, &res), "finish"); }
+    // offset of `need` bytes at `align` in the current arena, or in a fresh one when the arena or its extent table is full
+    uint64_t place(uint64_t align, uint64_t need)
+    {
+        const uint64_t o = align_up(s.pos, align);
+        if (o + need <= s.cap && s.room(1, 0))
+            return o;
+        submit();
+        acquire();
+        return 0;
+    }
+    uint64_t put(uint64_t o, uint64_t n, uint64_t suffix)
+    {
+        s.ext.push_back(mksnap_extent{o, n, suffix, MKSNAP_X_CRC, 0});
+        s.pos = o + n;
+        len.push_back(n);
+        return len.size() - 1;
+    }
+    // a path string, link target or prefix of n > 0 bytes; returns its extent
+    uint64_t text(const void *p, uint64_t n, uint64_t suffix)
+    {
+        if (n > s.cap)
+            throw HostError("path string larger than the arena");
+        const uint64_t o = place(16, n);
+        memcpy(s.a + o, p, n);
+        return put(o, n, suffix);
+    }
+    // the content of g, read into the arenas; with `after` (stream bytes behind the file) each piece's crc_suffix is the
+    // stream bytes behind that piece, without it 0 (only pure(piece) is wanted)
+    Sent file(const Seg &g, std::optional<uint64_t> after)
+    {
+        Sent f{&g, len.size(), 0};
+        for (uint64_t done = 0; done < g.size; ++f.n) {
+            const uint64_t o = place(512, 4096);
+            const uint64_t n = std::min<uint64_t>(g.size - done, (s.cap - o) / 16 * 16);
+            s.jobs.push_back(ReadJob{g.path, done, n, s.a + o});
+            done += n;
+            put(o, n, after ? *after + g.size - done : 0);
+        }
+        sent.push_back(f);
+        return f;
+    }
+    // after finish: pure(content) of every file that travelled into `cache` and / or `known`
+    void remember(mkhost_crc_cache *cache, std::map<FileKey, uint32_t> *known)
+    {
+        if (sent.empty() || !(cache || known))
+            return;
+        std::vector<uint32_t> pure(std::max<size_t>(1, len.size()));
+        uint64_t n_got = 0;
+        ck(s.eng, mksnap_get_extent_crcs(s.eng, pure.data(), pure.size(), &n_got), "extent crcs");
+        if (n_got != len.size())
+            throw HostError("internal: extent count mismatch");
+        for (const Sent &f : sent) { // pure(A||B) = pure(A) x^(8|B|) ^ pure(B)
+            uint32_t v = 0;          // pure of the empty string
+            for (uint64_t k = f.first; k < f.first + f.n; ++k)
+                v = mksnap_crc_concat(v, pure[k], len[k]);
+            if (cache)
+                cache->files[f.seg->path] = mkhost_crc_cache::Entry{f.seg->id, v};
+            if (known)
+                (*known)[file_key(*f.seg)] = v;
+        }
+    }
+};
+
+} // namespace
+
+extern "C" {
+
 static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc_cache_stats *stats, const void *prefix,
                               size_t prefix_len, const char *context_dir, const char *const *from_paths, size_t n_paths,
                               int n_threads, uint32_t *crc_out, uint64_t *stream_len_out, char *err, size_t errlen)
 {
     try {
-        const bool trace = getenv("MKHOST_TRACE") != nullptr; // phase times on stderr
         const auto t_start = std::chrono::steady_clock::now();
-        auto ms_since = [&](std::chrono::steady_clock::time_point t) {
-            return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t).count();
-        };
-        double ms_reads = 0, ms_submit = 0, ms_acquire = 0;
         std::vector<Seg> segs = context_segments(go_clean(context_dir), from_paths, n_paths, n_threads);
         const double ms_walk = ms_since(t_start);
         uint64_t total = prefix_len;
         for (const auto &g : segs)
             total += g.kind == 'F' ? g.size : g.bytes.size();
-        ArenaSession s(eng, n_threads, 1); // cap unrounded: CRC pieces end anywhere, files are cut at 16-byte granularity
-        auto t = std::chrono::steady_clock::now();
-        s.after_reads = [&]() {
-            ms_reads += ms_since(t);
-            t = std::chrono::steady_clock::now();
-        };
-        auto acquire = [&]() {
-            t = std::chrono::steady_clock::now();
-            s.acquire();
-            ms_acquire += ms_since(t);
-        };
-        auto flush = [&]() {
-            t = std::chrono::steady_clock::now();
-            s.submit();
-            ms_submit += ms_since(t);
-        };
-        ck(eng, mksnap_begin(eng), "begin");
-        acquire();
+        CrcPacker pk(eng, n_threads);
         uint64_t after = total; // stream bytes not yet placed
-        uint64_t n_crc_ext = 0; // CRC extents submitted so far in this session (index into mksnap_get_extent_crcs)
-        struct Sent {           // a file that travelled: its extents [first, first + pieces) and their lengths
-            const Seg *seg;
-            uint64_t first;
-            std::vector<uint64_t> piece_len;
-        };
-        std::vector<Sent> sent;
-        mkhost_crc_cache_stats st{};
-        auto put_bytes = [&](const void *p, size_t n) {
-            if (n == 0)
-                return;
-            uint64_t o = align_up(s.pos, 16);
-            if (o + n > s.cap || !s.room(1, 0)) {
-                flush();
-                acquire();
-                o = 0;
+        auto put_text = [&](const void *p, size_t n) {
+            if (n) {
+                after -= n;
+                pk.text(p, n, after);
             }
-            if (n > s.cap)
-                throw HostError("path string larger than the arena");
-            memcpy(s.a + o, p, n);
-            after -= n;
-            s.ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
-            ++n_crc_ext;
-            s.pos = o + n;
         };
-        put_bytes(prefix, prefix_len);
+        mkhost_crc_cache_stats st{};
+        put_text(prefix, prefix_len);
         for (const auto &g : segs) {
             if (g.kind != 'F') {
-                put_bytes(g.bytes.data(), g.bytes.size());
+                put_text(g.bytes.data(), g.bytes.size());
                 continue;
             }
             ++st.files_total;
             st.bytes_total += g.size;
+            after -= g.size;
             if (cache) { // unchanged since a build that remembered it: fold pure(content) in, send nothing
                 auto it = cache->files.find(g.path);
                 if (it != cache->files.end() && it->second.id == g.id) {
-                    after -= g.size;
                     ck(eng, mksnap_crc_add(eng, it->second.pure, g.size, after), "crc add");
                     ++st.files_reused;
                     continue;
                 }
             }
             st.bytes_sent += g.size;
-            if (cache)
-                sent.push_back(Sent{&g, n_crc_ext, {}});
-            uint64_t done = 0; // CRC is linear: a file may be split across arenas at any 16-byte boundary
-            while (done < g.size) {
-                uint64_t o = align_up(s.pos, 512);
-                if (o + 4096 > s.cap || !s.room(1, 0)) {
-                    flush();
-                    acquire();
-                    o = 0;
-                }
-                uint64_t n = std::min<uint64_t>(g.size - done, (s.cap - o) / 16 * 16);
-                s.jobs.push_back(ReadJob{g.path, done, n, s.a + o});
-                after -= n;
-                s.ext.push_back(mksnap_extent{o, n, after, MKSNAP_X_CRC, 0});
-                ++n_crc_ext;
-                if (cache)
-                    sent.back().piece_len.push_back(n);
-                s.pos = o + n;
-                done += n;
-            }
+            pk.file(g, after);
         }
-        flush();
+        pk.submit();
         mksnap_result res;
         const auto t_fin = std::chrono::steady_clock::now();
-        ck(eng, mksnap_finish(eng, &res), "finish");
-        if (trace)
+        pk.finish(res);
+        if (getenv("MKHOST_TRACE")) // phase times on stderr
             fprintf(stderr, "[mkhost] context crc32: %zu segments, %.1f MiB; walk %.2f ms, reads %.2f, acquire waits %.2f, submit %.2f, "
                             "finish %.2f, total %.2f ms\n",
-                    segs.size(), (double)total / 1048576.0, ms_walk, ms_reads, ms_acquire, ms_submit, ms_since(t_fin), ms_since(t_start));
+                    segs.size(), (double)total / 1048576.0, ms_walk, pk.ms_reads, pk.ms_acquire, pk.ms_submit, ms_since(t_fin),
+                    ms_since(t_start));
         if (res.crc_bytes != total)
             throw HostError("internal: stream length mismatch");
         *crc_out = mksnap_ctx_crc32(&res);
         if (stream_len_out)
             *stream_len_out = total;
-        if (cache) { // remember pure(content) of every file that travelled (pieces joined: pure(A||B) = pure(A) x^(8|B|) ^ pure(B))
-            std::vector<uint32_t> pure(std::max<uint64_t>(1, n_crc_ext));
-            uint64_t n_got = 0;
-            ck(eng, mksnap_get_extent_crcs(eng, pure.data(), pure.size(), &n_got), "extent crcs");
-            if (n_got != n_crc_ext)
-                throw HostError("internal: extent count mismatch");
-            for (const Sent &f : sent) {
-                uint32_t v = 0; // pure of the empty string
-                for (size_t k = 0; k < f.piece_len.size(); ++k)
-                    v = mksnap_crc_concat(v, pure[f.first + k], f.piece_len[k]);
-                cache->files[f.seg->path] = mkhost_crc_cache::Entry{f.seg->id, v};
-            }
-        }
+        pk.remember(cache, nullptr);
         if (stats)
             *stats = st;
         return 0;
@@ -1030,65 +1057,15 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
 // One engine session of mkhost_plan_cache_ids: the streams of the walked COPY/ADD steps `batch` (stream slot k = batch[k]).
 // Every distinct path string / link target and every file not yet valued travels once as CRC extents (crc_suffix 0:
 // only pure(extent) is wanted); each occurrence in a stream becomes a use of those extents, or of a known value.
-using FileKey = std::tuple<std::string, uint64_t, uint64_t, uint64_t, int64_t, int64_t>; // path, dev, ino, size, mtime, ctime
-static FileKey file_key(const Seg &g) { return FileKey{g.path, g.id.dev, g.id.ino, g.size, g.id.mtime_ns, g.id.ctime_ns}; }
-
 static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vector<std::vector<Seg>> &segs,
                          const std::vector<size_t> &batch, int n_threads, std::map<FileKey, uint32_t> &known,
                          bool remember, std::vector<uint32_t> &pure, std::vector<uint64_t> &slen,
                          mkhost_crc_cache_stats &st, double &ms_fold)
 {
-    ArenaSession s(eng, n_threads, 1); // cap unrounded, as in the single-step pass
-    ck(eng, mksnap_begin(eng), "begin");
-    s.acquire();
-    uint64_t n_ext = 0; // CRC extents submitted so far (mksnap_get_extent_crcs numbering)
-    auto place = [&](uint64_t align, uint64_t need) {
-        uint64_t o = align_up(s.pos, align);
-        if (o + need > s.cap || !s.room(1, 0)) {
-            s.submit();
-            s.acquire();
-            o = 0;
-        }
-        return o;
-    };
-    std::map<std::string, uint64_t> text_ext; // path string / link target -> its extent
-    auto put_text = [&](const std::string &b) {
-        auto it = text_ext.find(b);
-        if (it != text_ext.end())
-            return it->second;
-        if (b.size() > s.cap)
-            throw HostError("path string larger than the arena");
-        const uint64_t o = place(16, b.size());
-        memcpy(s.a + o, b.data(), b.size());
-        s.ext.push_back(mksnap_extent{o, b.size(), 0, MKSNAP_X_CRC, 0});
-        s.pos = o + b.size();
-        text_ext.emplace(b, n_ext);
-        return n_ext++;
-    };
-    struct Sent { // a file that travelled: extents [first, first + pieces) and their lengths
-        const Seg *seg;
-        uint64_t first;
-        std::vector<uint64_t> piece_len;
-    };
-    std::vector<Sent> sent;
-    std::map<FileKey, size_t> sent_of;
-    auto put_file = [&](const Seg &g) { // CRC is linear: a file may be split across arenas at any 16-byte boundary
-        Sent f{&g, n_ext, {}};
-        for (uint64_t done = 0; done < g.size;) {
-            const uint64_t o = place(512, 4096);
-            const uint64_t n = std::min<uint64_t>(g.size - done, (s.cap - o) / 16 * 16);
-            s.jobs.push_back(ReadJob{g.path, done, n, s.a + o});
-            s.ext.push_back(mksnap_extent{o, n, 0, MKSNAP_X_CRC, 0});
-            ++n_ext;
-            f.piece_len.push_back(n);
-            s.pos = o + n;
-            done += n;
-        }
-        st.bytes_sent += g.size;
-        sent.push_back(std::move(f));
-        return sent.size() - 1;
-    };
-    std::vector<mksnap_crc_use> uses; // grouped by stream, as k_crc_fold prefers them
+    CrcPacker pk(eng, n_threads);
+    std::map<std::string, uint64_t> text_ext;   // path string / link target -> its extent
+    std::map<FileKey, CrcPacker::Sent> sent_of; // file -> its extents
+    std::vector<mksnap_crc_use> uses;           // grouped by stream, as k_crc_fold prefers them
     for (size_t k = 0; k < batch.size(); ++k) {
         const uint32_t slot = (uint32_t)k;
         const std::vector<Seg> &ss = segs[batch[k]];
@@ -1099,8 +1076,12 @@ static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vect
         for (const auto &g : ss) {
             if (g.kind != 'F') {
                 after -= g.bytes.size();
-                if (!g.bytes.empty())
-                    uses.push_back(mksnap_crc_use{after, put_text(g.bytes), slot, 0});
+                if (g.bytes.empty())
+                    continue;
+                auto it = text_ext.find(g.bytes);
+                if (it == text_ext.end())
+                    it = text_ext.emplace(g.bytes, pk.text(g.bytes.data(), g.bytes.size(), 0)).first;
+                uses.push_back(mksnap_crc_use{after, it->second, slot, 0});
                 continue;
             }
             ++st.files_total;
@@ -1123,43 +1104,31 @@ static void plan_session(mksnap_t *eng, mkhost_crc_cache *cache, const std::vect
                 continue;
             }
             auto so = sent_of.find(key);
-            const Sent &f = sent[so != sent_of.end() ? so->second : (sent_of[key] = put_file(g))];
+            if (so == sent_of.end()) {
+                so = sent_of.emplace(key, pk.file(g, std::nullopt)).first;
+                st.bytes_sent += g.size;
+            }
+            const CrcPacker::Sent &f = so->second;
             uint64_t a = after + g.size;
-            for (size_t p = 0; p < f.piece_len.size(); ++p) {
-                a -= f.piece_len[p];
-                uses.push_back(mksnap_crc_use{a, f.first + p, slot, 0});
+            for (uint64_t x = f.first; x < f.first + f.n; ++x) {
+                a -= pk.len[x];
+                uses.push_back(mksnap_crc_use{a, x, slot, 0});
             }
         }
     }
-    s.submit();
+    pk.submit();
     const auto t_fold = std::chrono::steady_clock::now();
-    for (size_t u0 = 0; u0 < uses.size(); u0 += s.lim.max_extents)
-        ck(eng, mksnap_crc_fold(eng, uses.data() + u0, std::min<uint64_t>(s.lim.max_extents, uses.size() - u0)), "crc fold");
+    for (size_t u0 = 0; u0 < uses.size(); u0 += pk.s.lim.max_extents)
+        ck(eng, mksnap_crc_fold(eng, uses.data() + u0, std::min<uint64_t>(pk.s.lim.max_extents, uses.size() - u0)), "crc fold");
     mksnap_result res;
-    ck(eng, mksnap_finish(eng, &res), "finish");
-    ms_fold += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_fold).count();
+    pk.finish(res);
+    ms_fold += ms_since(t_fold);
     std::vector<uint32_t> val(batch.size());
     uint64_t n_val = 0;
     ck(eng, mksnap_get_crc_streams(eng, val.data(), val.size(), &n_val), "crc streams");
     for (size_t k = 0; k < batch.size(); ++k)
         pure[batch[k]] = k < n_val ? val[k] : 0u; // a stream nothing was folded into is empty
-    if (sent.empty() || !(cache || remember))
-        return;
-    std::vector<uint32_t> ext(n_ext);
-    uint64_t n_got = 0;
-    ck(eng, mksnap_get_extent_crcs(eng, ext.data(), ext.size(), &n_got), "extent crcs");
-    if (n_got != n_ext)
-        throw HostError("internal: extent count mismatch");
-    for (const Sent &f : sent) { // pure(A||B) = pure(A) x^(8|B|) ^ pure(B)
-        uint32_t v = 0;
-        for (size_t p = 0; p < f.piece_len.size(); ++p)
-            v = mksnap_crc_concat(v, ext[f.first + p], f.piece_len[p]);
-        const Seg &g = *f.seg;
-        if (cache)
-            cache->files[g.path] = mkhost_crc_cache::Entry{g.id, v};
-        if (remember)
-            known[file_key(g)] = v;
-    }
+    pk.remember(cache, remember ? &known : nullptr);
 }
 
 int mkhost_plan_cache_ids(mksnap_t *eng, mkhost_crc_cache *cache, const char *seed, const char *context_dir,
@@ -1184,7 +1153,7 @@ int mkhost_plan_cache_ids(mksnap_t *eng, mkhost_crc_cache *cache, const char *se
                 walked.push_back(i);
             }
         }
-        const double ms_walk = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count();
+        const double ms_walk = ms_since(t_start);
         std::vector<uint32_t> pure(n_steps, 0);
         std::vector<uint64_t> slen(n_steps, 0);
         mkhost_crc_cache_stats st{};
@@ -1223,8 +1192,7 @@ int mkhost_plan_cache_ids(mksnap_t *eng, mkhost_crc_cache *cache, const char *se
         }
         if (getenv("MKHOST_TRACE"))
             fprintf(stderr, "[mkhost] plan cacheIDs: %zu steps, %zu walked, %zu sessions; walk %.2f ms, fold + finish %.2f ms, total %.2f ms\n",
-                    n_steps, walked.size(), n_sessions, ms_walk, ms_fold,
-                    std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_start).count());
+                    n_steps, walked.size(), n_sessions, ms_walk, ms_fold, ms_since(t_start));
         if (stats)
             *stats = st;
         return 0;
