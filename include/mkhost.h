@@ -209,7 +209,8 @@ int mkhost_memfs_commit_scan(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, i
  * The reference commits layer by layer (build_node.go:102-107); COPY/ADD steps that do not modify the file system
  * (no RUN in between) can be deferred and committed together, which is what a cgo caller would do (INTEGRATION.md).
  * outs[i].tar_digest / tar_bytes / n_entries are per layer; root / n_chunks / n_unique describe the chunk table of the
- * whole batch (one session).  flags: MKHOST_NO_TAR_DIGEST only.  tar_fd < 0: that layer's tar is not emitted. */
+ * whole batch (one session).  flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS.  tar_fd < 0: that layer's tar is not
+ * emitted.  This is mkhost_memfs_commit_layers_cached with cache == NULL. */
 typedef struct {
     const mkhost_copy_op *ops;
     size_t n_ops;
@@ -218,6 +219,24 @@ typedef struct {
 int mkhost_memfs_commit_layers(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_layer_spec *layers,
                                size_t n_layers, int n_threads, uint32_t flags, mkhost_layer_result *outs, char *err,
                                size_t errlen);
+/* Batched incremental layer commit.  The result equals calling mkhost_memfs_commit_copy_ops_cached once per layer, in
+ * order, with the same cache and flags: the same tree and the same remembered file digests (a destination written by
+ * two layers keeps the later layer's digest), the same bytes to each layer's tar_fd, the same outs[i].tar_digest,
+ * n_entries and tar_bytes, and the same cache contents afterwards (mkhost_chunk_cache_save writes the same bytes).  Two
+ * things differ by design: outs[i].root / n_chunks / n_unique describe the chunk table of the whole batch, as for
+ * mkhost_memfs_commit_layers; and every lookup uses the cache as it stood when the call started, so a source that two
+ * layers copy and the cache does not yet hold is chunked in both (the table is sorted and unique: the root is the
+ * same).  stats adds up over the batch and counts every occurrence of a file (files_reused included).  cache == NULL:
+ * no cache.  flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS; any other flag is refused.
+ * Stream slots: layer i's TarDigest chain is slot i; under MKHOST_FILE_DIGESTS every regular file with content in the
+ * batch takes one slot from n_layers on.  A batch whose layers plus such files exceed mksnap_limits.max_streams is
+ * refused before anything is read or submitted.
+ * Deliberately not supported: an entry larger than one arena is refused ("exceeds the arena"), since it would have to
+ * stay open across submits next to the other layers' pieces; and MKHOST_MATERIALIZE, since the copier mode (--chown or
+ * not) belongs to each step and mkhost_layer_spec has no field for it. */
+int mkhost_memfs_commit_layers_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chunk_cache *cache, int64_t now_unix,
+                                      const mkhost_layer_spec *layers, size_t n_layers, int n_threads, uint32_t flags,
+                                      mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err, size_t errlen);
 /* the same two without a GPU: entry list as text (format below); they DO merge the layer into the tree */
 size_t mkhost_memfs_describe_copy_ops(mkhost_memfs *m, int64_t now_unix, const mkhost_copy_op *ops, size_t n_ops, char *out,
                                       size_t cap, char *err, size_t errlen);

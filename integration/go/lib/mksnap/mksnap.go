@@ -224,7 +224,62 @@ func (fs *MemFS) CommitScan(e *Engine, now int64, tarOut *os.File, threads int, 
 
 // CommitLayers commits consecutive COPY/ADD layers of one build in ONE engine session: every TarDigest chain
 // advances together on the device (on an H100 one chain runs at ~0.06 GB/s, 256 chains at ~15 GB/s).  tarOuts[i] may be nil.
+// flags: NoTarDigest, FileDigests.
 func (fs *MemFS) CommitLayers(e *Engine, now int64, layers [][]CopyOp, tarOuts []*os.File, threads int, flags uint32) ([]LayerResult, error) {
+	res, _, err := fs.CommitLayersCached(e, nil, now, layers, tarOuts, threads, flags)
+	return res, err
+}
+
+// ChunkCache remembers the chunk digests of every source file a layer commit chunked (include/mkhost.h, "Incremental
+// layer commit"): an unchanged file (same device, inode, size, mtime, ctime) is not chunked again, and under
+// NoTarDigest its bytes do not travel to the device.  One cache per build context; Save/Load keep it between makisu
+// invocations.
+type ChunkCache struct{ c *C.mkhost_chunk_cache }
+
+// NewChunkCache loads `path` when it exists ("" = start cold).
+func NewChunkCache(path string) (*ChunkCache, error) {
+	cc := &ChunkCache{c: C.mkhost_chunk_cache_new()}
+	runtime.SetFinalizer(cc, func(cc *ChunkCache) { C.mkhost_chunk_cache_free(cc.c) })
+	if path == "" {
+		return cc, nil
+	}
+	if _, err := os.Stat(path); err != nil {
+		return cc, nil
+	}
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_chunk_cache_load(cc.c, cpath, errBuf, errLen) != 0 {
+		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return cc, nil
+}
+
+// Save writes the cache next to the build context (or into makisu's storage dir).
+func (cc *ChunkCache) Save(path string) error {
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cpath := C.CString(path)
+	defer C.free(unsafe.Pointer(cpath))
+	if C.mkhost_chunk_cache_save(cc.c, cpath, errBuf, errLen) != 0 {
+		return fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return nil
+}
+
+// ChunkCacheStats adds up over a call: regular files and their bytes, files taken from the cache, bytes chunked on
+// the device, file bytes copied to the device.
+type ChunkCacheStats struct {
+	FilesTotal, FilesReused                 uint64
+	BytesTotal, BytesChunked, BytesUploaded uint64
+}
+
+// CommitLayersCached is CommitLayers with the chunk cache in the loop (cc == nil: no cache).  The result equals one
+// cached commit per layer in order -- tree, file digests, tar bytes, TarDigest per layer, the cache afterwards --
+// except that every lookup sees the cache as it was when the call started.
+func (fs *MemFS) CommitLayersCached(e *Engine, cc *ChunkCache, now int64, layers [][]CopyOp, tarOuts []*os.File, threads int,
+	flags uint32) ([]LayerResult, ChunkCacheStats, error) {
 	n := len(layers)
 	specs := (*C.mkhost_layer_spec)(C.calloc(C.size_t(n+1), C.size_t(unsafe.Sizeof(C.mkhost_layer_spec{}))))
 	defer C.free(unsafe.Pointer(specs))
@@ -241,16 +296,22 @@ func (fs *MemFS) CommitLayers(e *Engine, now int64, layers [][]CopyOp, tarOuts [
 	defer C.free(unsafe.Pointer(outs))
 	errBuf := (*C.char)(C.malloc(errLen))
 	defer C.free(unsafe.Pointer(errBuf))
-	if rc := C.mkhost_memfs_commit_layers(fs.m, e.h, C.int64_t(now), specs, C.size_t(n), C.int(threads), C.uint32_t(flags),
-		outs, errBuf, errLen); rc != 0 {
-		return nil, fmt.Errorf("%s", C.GoString(errBuf))
+	var cache *C.mkhost_chunk_cache
+	if cc != nil {
+		cache = cc.c
+	}
+	var st C.mkhost_chunk_cache_stats
+	if rc := C.mkhost_memfs_commit_layers_cached(fs.m, e.h, cache, C.int64_t(now), specs, C.size_t(n), C.int(threads),
+		C.uint32_t(flags), outs, &st, errBuf, errLen); rc != 0 {
+		return nil, ChunkCacheStats{}, fmt.Errorf("%s", C.GoString(errBuf))
 	}
 	oview := (*[1 << 20]C.mkhost_layer_result)(unsafe.Pointer(outs))[:n:n]
 	res := make([]LayerResult, n)
 	for i := range res {
 		res[i] = toResult(&oview[i])
 	}
-	return res, nil
+	return res, ChunkCacheStats{uint64(st.files_total), uint64(st.files_reused), uint64(st.bytes_total),
+		uint64(st.bytes_chunked), uint64(st.bytes_uploaded)}, nil
 }
 
 // DecodesInParallel reports whether the gzip blob in f has, in its first 2 MiB, segment starts that let the device

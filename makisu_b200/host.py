@@ -99,6 +99,9 @@ SYMBOLS = [
                                                       C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_commit_layers", C.c_int, [_P, _P, C.c_int64, C.POINTER(LayerSpec), C.c_size_t, C.c_int, C.c_uint32,
                                              C.POINTER(LayerResult), C.c_char_p, C.c_size_t]),
+    ("mkhost_memfs_commit_layers_cached", C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(LayerSpec), C.c_size_t, C.c_int,
+                                                    C.c_uint32, C.POINTER(LayerResult), C.POINTER(ChunkCacheStats),
+                                                    C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_commit_scan", C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, C.c_uint32, C.POINTER(LayerResult),
                                            C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_describe_copy_ops", C.c_size_t, [_P, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_char_p, C.c_size_t,
@@ -396,7 +399,26 @@ class MemFS:
 
     def commit_layers(self, eng: abi.Engine, now_unix: int, layers: Sequence[Sequence[CopyOperation]], n_threads: int = 0,
                       tar_fds: Optional[Sequence[int]] = None, flags: int = 0):
-        """Consecutive layers of one build in ONE engine session (all TarDigest chains advance together)."""
+        """Consecutive layers of one build in ONE engine session (all TarDigest chains advance together).
+        flags: MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS."""
+        return self._commit_layers(layers, tar_fds, lambda specs, n, outs, err: load().mkhost_memfs_commit_layers(
+            self.h, eng.h, now_unix, specs, n, n_threads, flags, outs, err, len(err)))
+
+    def commit_layers_cached(self, eng: abi.Engine, cache: Optional["ChunkCache"], now_unix: int,
+                             layers: Sequence[Sequence[CopyOperation]], n_threads: int = 0,
+                             tar_fds: Optional[Sequence[int]] = None, flags: int = 0):
+        """commit_layers with remembered chunk digests for unchanged files -> (layer dicts, stats dict summed over the
+        batch).  Equals commit_copy_ops_cached once per layer, except root / n_chunks / n_unique (the whole batch's) and
+        the cache lookups, which all see the cache as it was when the call started.  cache None = no cache."""
+        st = ChunkCacheStats()
+        res = self._commit_layers(layers, tar_fds, lambda specs, n, outs, err: load().mkhost_memfs_commit_layers_cached(
+            self.h, eng.h, cache.h if cache is not None else None, now_unix, specs, n, n_threads, flags, outs, C.byref(st),
+            err, len(err)))
+        return res, {k: getattr(st, k) for k, _ in ChunkCacheStats._fields_}
+
+    @staticmethod
+    def _commit_layers(layers: Sequence[Sequence[CopyOperation]], tar_fds: Optional[Sequence[int]], call) -> List[dict]:
+        """call(specs, n, outs, err) makes the C call -> one result dict per layer."""
         err = C.create_string_buffer(1024)
         n = len(layers)
         specs, keep, outs = (LayerSpec * max(1, n))(), [], (LayerResult * max(1, n))()
@@ -405,7 +427,7 @@ class MemFS:
             keep.append((arr, k))
             specs[i].ops, specs[i].n_ops = arr, len(ops)
             specs[i].tar_fd = tar_fds[i] if tar_fds is not None else -1
-        if load().mkhost_memfs_commit_layers(self.h, eng.h, now_unix, specs, n, n_threads, flags, outs, err, len(err)):
+        if call(specs, n, outs, err):
             raise HostError(err.value.decode())
         return [_layer_dict(outs[i]) for i in range(n)]
 

@@ -460,11 +460,19 @@ int mkhost_memfs_commit_copy_ops_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_c
 int mkhost_memfs_commit_layers(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, const mkhost_layer_spec *specs, size_t n_layers,
                                int n_threads, uint32_t flags, mkhost_layer_result *outs, char *err, size_t errlen)
 {
+    return mkhost_memfs_commit_layers_cached(m, eng, nullptr, now_unix, specs, n_layers, n_threads, flags, outs, nullptr, err,
+                                             errlen);
+}
+
+int mkhost_memfs_commit_layers_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chunk_cache *cache, int64_t now_unix,
+                                      const mkhost_layer_spec *specs, size_t n_layers, int n_threads, uint32_t flags,
+                                      mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err, size_t errlen)
+{
     try {
         if (!m || !eng || (!specs && n_layers) || (!outs && n_layers))
             throw HostError("null argument");
-        if (flags & ~(uint32_t)MKHOST_NO_TAR_DIGEST)
-            throw HostError("commit layers: only MKHOST_NO_TAR_DIGEST is supported for a batch");
+        if (flags & ~(uint32_t)(MKHOST_NO_TAR_DIGEST | MKHOST_FILE_DIGESTS))
+            throw HostError("commit layers: only MKHOST_NO_TAR_DIGEST and MKHOST_FILE_DIGESTS are supported for a batch");
         m->fs.set_now(now_unix);
         // the layer maps are built in order -- each AddLayerByCopyOps sees the tree its predecessors left
         // (mem_fs.go:276-289) -- and only then packed together
@@ -475,7 +483,7 @@ int mkhost_memfs_commit_layers(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix,
         std::vector<BatchLayer> bl;
         for (size_t i = 0; i < n_layers; ++i)
             bl.push_back(BatchLayer{&maps[i], specs[i].tar_fd});
-        commit_layers_batch(eng, bl, n_threads, flags, outs);
+        commit_layers_batch(eng, bl, n_threads, flags, outs, &m->fs, cache ? &cache->memo : nullptr, stats);
         return 0;
     } catch (const std::exception &e) {
         set_err(err, errlen, std::string("failed to generate diff layers: ") + e.what());
