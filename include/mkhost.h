@@ -94,6 +94,20 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
                                 uint32_t *crc_out, uint64_t *stream_len_out, mkhost_crc_cache_stats *stats, char *err,
                                 size_t errlen);
 
+/* Several engines (mksnap handles: one per GPU, or several on one) driven from one call.  The engines' handles must not be
+ * used by anything else during the call; each is driven from a thread of its own, which the engine allows for different
+ * handles.  mkhost_context_crc32_multi returns what mkhost_context_crc32_cached(engines[0], ...) returns for the whole
+ * context -- crc_out, stream_len_out, stats and the cache contents afterwards, bit for bit -- and with n_engines == 1 it
+ * is that call.  cache may be NULL (no cache).  The context is walked once; every segment's crc_suffix is its place in
+ * the whole stream, so each engine's crc_pure is its share of the value and the shares XOR.  Files that travel are
+ * assigned whole to the engines by LPT over their bytes; a path string or link target goes with the next file that
+ * travels, or to engine 0, which also takes the prefix and folds every file the cache vouches for.  Each engine packs
+ * on its own thread with its own pool of n_threads readers.  An engine given nothing is not used. */
+int mkhost_context_crc32_multi(mksnap_t *const *engines, size_t n_engines, mkhost_crc_cache *cache, const void *prefix,
+                               size_t prefix_len, const char *context_dir, const char *const *from_paths, size_t n_paths,
+                               int n_threads, uint32_t *crc_out, uint64_t *stream_len_out, mkhost_crc_cache_stats *stats,
+                               char *err, size_t errlen);
+
 /* cacheID of every step of a build plan (processStagesAndAliases + createDockerfileSteps, lib/builder/build_plan.go:93-160,
  * build_stage.go:153-165: each step is seeded with the cacheID of the step before it), with the context read once for
  * the whole plan.  The sources of every COPY/ADD step are walked like mkhost_context_crc32 walks them; a file that
@@ -237,6 +251,22 @@ int mkhost_memfs_commit_layers(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix,
 int mkhost_memfs_commit_layers_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chunk_cache *cache, int64_t now_unix,
                                       const mkhost_layer_spec *layers, size_t n_layers, int n_threads, uint32_t flags,
                                       mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err, size_t errlen);
+/* mkhost_memfs_commit_layers_cached with the layers shared out over n_engines engines (see mkhost_context_crc32_multi
+ * for the threading).  The result equals that of mkhost_memfs_commit_layers_cached(m, engines[0], cache, ...) with the
+ * same layers, cache and flags: every layer's bytes to its tar_fd, outs[i].tar_digest, n_entries and tar_bytes, the
+ * batch's root / n_chunks / n_unique in every outs[i], the tree and its remembered file digests (a destination written
+ * by two layers keeps the later layer's digest, whichever engines hashed them), stats, and the bytes
+ * mkhost_chunk_cache_save writes afterwards; with n_engines == 1 it is that call.  Layers, not entries, are assigned to
+ * the engines, by LPT over their tar bytes; each engine commits its share as one batch in a session of its own, with
+ * stream slots counted per engine (a share its engine cannot hold is refused before any engine reads or submits).
+ * Engines 1..N-1 finish first and their sorted-unique tables join engine 0's session (mksnap_chunks_add), whose finish
+ * sorts, uniques and roots the union: it must fit engine 0's max_chunks (else its MKSNAP_E_CAPACITY message, and the
+ * cache records nothing).  Lookups see the cache as the call found it; what the engines chunked is recorded once all
+ * have finished.  The engines must cut under the same CDC parameters. */
+int mkhost_memfs_commit_layers_multi(mkhost_memfs *m, mksnap_t *const *engines, size_t n_engines, mkhost_chunk_cache *cache,
+                                     int64_t now_unix, const mkhost_layer_spec *layers, size_t n_layers, int n_threads,
+                                     uint32_t flags, mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err,
+                                     size_t errlen);
 /* the same two without a GPU: entry list as text (format below); they DO merge the layer into the tree */
 size_t mkhost_memfs_describe_copy_ops(mkhost_memfs *m, int64_t now_unix, const mkhost_copy_op *ops, size_t n_ops, char *out,
                                       size_t cap, char *err, size_t errlen);

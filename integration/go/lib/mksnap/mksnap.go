@@ -280,6 +280,26 @@ type ChunkCacheStats struct {
 // except that every lookup sees the cache as it was when the call started.
 func (fs *MemFS) CommitLayersCached(e *Engine, cc *ChunkCache, now int64, layers [][]CopyOp, tarOuts []*os.File, threads int,
 	flags uint32) ([]LayerResult, ChunkCacheStats, error) {
+	return fs.CommitLayersMulti([]*Engine{e}, cc, now, layers, tarOuts, threads, flags)
+}
+
+// engineArray is the mksnap_t * of every engine in C memory; free it with C.free.
+func engineArray(engines []*Engine) **C.mksnap_t {
+	n := len(engines)
+	arr := (**C.mksnap_t)(C.calloc(C.size_t(n+1), C.size_t(unsafe.Sizeof((*C.mksnap_t)(nil)))))
+	view := (*[1 << 20]*C.mksnap_t)(unsafe.Pointer(arr))[:n:n]
+	for i, e := range engines {
+		view[i] = e.h
+	}
+	return arr
+}
+
+// CommitLayersMulti is CommitLayersCached with the layers shared out over several engines -- one per GPU of the build
+// host, or several on one -- each driven by libmkhost from a thread of its own (mkhost_memfs_commit_layers_multi).  The
+// result is that of CommitLayersCached on engines[0], bit for bit.  The engines must not be used by anything else
+// during the call.
+func (fs *MemFS) CommitLayersMulti(engines []*Engine, cc *ChunkCache, now int64, layers [][]CopyOp, tarOuts []*os.File,
+	threads int, flags uint32) ([]LayerResult, ChunkCacheStats, error) {
 	n := len(layers)
 	specs := (*C.mkhost_layer_spec)(C.calloc(C.size_t(n+1), C.size_t(unsafe.Sizeof(C.mkhost_layer_spec{}))))
 	defer C.free(unsafe.Pointer(specs))
@@ -300,9 +320,11 @@ func (fs *MemFS) CommitLayersCached(e *Engine, cc *ChunkCache, now int64, layers
 	if cc != nil {
 		cache = cc.c
 	}
+	hs := engineArray(engines)
+	defer C.free(unsafe.Pointer(hs))
 	var st C.mkhost_chunk_cache_stats
-	if rc := C.mkhost_memfs_commit_layers_cached(fs.m, e.h, cache, C.int64_t(now), specs, C.size_t(n), C.int(threads),
-		C.uint32_t(flags), outs, &st, errBuf, errLen); rc != 0 {
+	if rc := C.mkhost_memfs_commit_layers_multi(fs.m, hs, C.size_t(len(engines)), cache, C.int64_t(now), specs, C.size_t(n),
+		C.int(threads), C.uint32_t(flags), outs, &st, errBuf, errLen); rc != 0 {
 		return nil, ChunkCacheStats{}, fmt.Errorf("%s", C.GoString(errBuf))
 	}
 	oview := (*[1 << 20]C.mkhost_layer_result)(unsafe.Pointer(outs))[:n:n]
@@ -414,6 +436,38 @@ func (e *Engine) ContextCRC32Cached(cc *CrcCache, prefix []byte, contextDir stri
 	}
 	if rc := C.mkhost_context_crc32_cached(e.h, cc.c, p, C.size_t(len(prefix)), cdir, paths, C.size_t(len(fromPaths)),
 		C.int(threads), &c, &n, &st, errBuf, errLen); rc != 0 {
+		return 0, 0, fmt.Errorf("%s", C.GoString(errBuf))
+	}
+	return uint32(c), uint64(st.bytes_sent), nil
+}
+
+// ContextCRC32Multi is ContextCRC32Cached with the context's files shared out over several engines, each driven by
+// libmkhost from a thread of its own (mkhost_context_crc32_multi); cc may be nil.  The cacheID is that of one engine,
+// bit for bit.
+func ContextCRC32Multi(engines []*Engine, cc *CrcCache, prefix []byte, contextDir string, fromPaths []string,
+	threads int) (crc uint32, sent uint64, err error) {
+	var c C.uint32_t
+	var n C.uint64_t
+	var st C.mkhost_crc_cache_stats
+	errBuf := (*C.char)(C.malloc(errLen))
+	defer C.free(unsafe.Pointer(errBuf))
+	cdir := C.CString(contextDir)
+	defer C.free(unsafe.Pointer(cdir))
+	paths, free := cStrings(fromPaths)
+	defer free()
+	var p unsafe.Pointer
+	if len(prefix) > 0 {
+		p = C.CBytes(prefix)
+		defer C.free(p)
+	}
+	var cache *C.mkhost_crc_cache
+	if cc != nil {
+		cache = cc.c
+	}
+	hs := engineArray(engines)
+	defer C.free(unsafe.Pointer(hs))
+	if rc := C.mkhost_context_crc32_multi(hs, C.size_t(len(engines)), cache, p, C.size_t(len(prefix)), cdir, paths,
+		C.size_t(len(fromPaths)), C.int(threads), &c, &n, &st, errBuf, errLen); rc != 0 {
 		return 0, 0, fmt.Errorf("%s", C.GoString(errBuf))
 	}
 	return uint32(c), uint64(st.bytes_sent), nil

@@ -76,6 +76,9 @@ SYMBOLS = [
     ("mkhost_context_crc32_cached", C.c_int, [_P, _P, _P, C.c_size_t, C.c_char_p, C.POINTER(C.c_char_p), C.c_size_t, C.c_int,
                                               C.POINTER(C.c_uint32), C.POINTER(C.c_uint64), C.POINTER(CrcCacheStats), C.c_char_p,
                                               C.c_size_t]),
+    ("mkhost_context_crc32_multi", C.c_int, [C.POINTER(_P), C.c_size_t, _P, _P, C.c_size_t, C.c_char_p, C.POINTER(C.c_char_p),
+                                             C.c_size_t, C.c_int, C.POINTER(C.c_uint32), C.POINTER(C.c_uint64),
+                                             C.POINTER(CrcCacheStats), C.c_char_p, C.c_size_t]),
     ("mkhost_plan_cache_ids", C.c_int, [_P, _P, C.c_char_p, C.c_char_p, C.POINTER(_PlanStep), C.c_size_t, C.c_int,
                                         C.POINTER(C.c_uint32), C.POINTER(CrcCacheStats), C.c_char_p, C.c_size_t]),
     ("mkhost_commit_copy_ops", C.c_int, [_P, C.c_char_p, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_int,
@@ -102,6 +105,9 @@ SYMBOLS = [
     ("mkhost_memfs_commit_layers_cached", C.c_int, [_P, _P, _P, C.c_int64, C.POINTER(LayerSpec), C.c_size_t, C.c_int,
                                                     C.c_uint32, C.POINTER(LayerResult), C.POINTER(ChunkCacheStats),
                                                     C.c_char_p, C.c_size_t]),
+    ("mkhost_memfs_commit_layers_multi", C.c_int, [_P, C.POINTER(_P), C.c_size_t, _P, C.c_int64, C.POINTER(LayerSpec),
+                                                   C.c_size_t, C.c_int, C.c_uint32, C.POINTER(LayerResult),
+                                                   C.POINTER(ChunkCacheStats), C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_commit_scan", C.c_int, [_P, _P, C.c_int64, C.c_int, C.c_int, C.c_uint32, C.POINTER(LayerResult),
                                            C.c_char_p, C.c_size_t]),
     ("mkhost_memfs_describe_copy_ops", C.c_size_t, [_P, C.c_int64, C.POINTER(CopyOp), C.c_size_t, C.c_char_p, C.c_size_t,
@@ -244,6 +250,24 @@ def context_crc32(eng: abi.Engine, prefix: bytes, context_dir: str, from_paths: 
     if rc:
         raise HostError(err.value.decode())
     return crc.value, slen.value
+
+
+def _engines(engines: Sequence[abi.Engine]):
+    return (_P * max(1, len(engines)))(*[e.h for e in engines])
+
+
+def context_crc32_multi(engines: Sequence[abi.Engine], prefix: bytes, context_dir: str, from_paths: Sequence[str],
+                        n_threads: int = 0, cache: Optional["CrcCache"] = None):
+    """context_crc32 (with `cache`: CrcCache.context_crc32) with the files sharded over several engines, each driven
+    from a thread of its own -> (crc32, stream length, stats dict).  Bit for bit the single-engine result."""
+    err = C.create_string_buffer(1024)
+    crc, slen, st = C.c_uint32(), C.c_uint64(), CrcCacheStats()
+    rc = load().mkhost_context_crc32_multi(_engines(engines), len(engines), cache.h if cache is not None else None, prefix,
+                                           len(prefix), os.fsencode(context_dir), _strs(from_paths), len(from_paths),
+                                           n_threads, C.byref(crc), C.byref(slen), C.byref(st), err, len(err))
+    if rc:
+        raise HostError(err.value.decode())
+    return crc.value, slen.value, {k: getattr(st, k) for k, _ in CrcCacheStats._fields_}
 
 
 def copy_step_cache_id(eng: abi.Engine, seed: str, directive: str, args: str, context_dir: str,
@@ -414,6 +438,17 @@ class MemFS:
         res = self._commit_layers(layers, tar_fds, lambda specs, n, outs, err: load().mkhost_memfs_commit_layers_cached(
             self.h, eng.h, cache.h if cache is not None else None, now_unix, specs, n, n_threads, flags, outs, C.byref(st),
             err, len(err)))
+        return res, {k: getattr(st, k) for k, _ in ChunkCacheStats._fields_}
+
+    def commit_layers_multi(self, engines: Sequence[abi.Engine], cache: Optional["ChunkCache"], now_unix: int,
+                            layers: Sequence[Sequence[CopyOperation]], n_threads: int = 0,
+                            tar_fds: Optional[Sequence[int]] = None, flags: int = 0):
+        """commit_layers_cached with the layers sharded over several engines, each driven from a thread of its own ->
+        (layer dicts, stats dict).  The result is that of commit_layers_cached on engines[0]; cache None = no cache."""
+        st, hs = ChunkCacheStats(), _engines(engines)
+        res = self._commit_layers(layers, tar_fds, lambda specs, n, outs, err: load().mkhost_memfs_commit_layers_multi(
+            self.h, hs, len(engines), cache.h if cache is not None else None, now_unix, specs, n, n_threads, flags, outs,
+            C.byref(st), err, len(err)))
         return res, {k: getattr(st, k) for k, _ in ChunkCacheStats._fields_}
 
     @staticmethod

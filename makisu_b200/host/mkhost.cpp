@@ -22,6 +22,7 @@
 #include <array>
 #include <atomic>
 #include <condition_variable>
+#include <exception>
 #include <functional>
 #include <map>
 #include <memory>
@@ -468,9 +469,21 @@ int mkhost_memfs_commit_layers_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chu
                                       const mkhost_layer_spec *specs, size_t n_layers, int n_threads, uint32_t flags,
                                       mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err, size_t errlen)
 {
+    return mkhost_memfs_commit_layers_multi(m, &eng, 1, cache, now_unix, specs, n_layers, n_threads, flags, outs, stats, err,
+                                            errlen);
+}
+
+int mkhost_memfs_commit_layers_multi(mkhost_memfs *m, mksnap_t *const *engines, size_t n_engines, mkhost_chunk_cache *cache,
+                                     int64_t now_unix, const mkhost_layer_spec *specs, size_t n_layers, int n_threads,
+                                     uint32_t flags, mkhost_layer_result *outs, mkhost_chunk_cache_stats *stats, char *err,
+                                     size_t errlen)
+{
     try {
-        if (!m || !eng || (!specs && n_layers) || (!outs && n_layers))
+        if (!m || !engines || n_engines == 0 || (!specs && n_layers) || (!outs && n_layers))
             throw HostError("null argument");
+        for (size_t k = 0; k < n_engines; ++k)
+            if (!engines[k])
+                throw HostError("null argument");
         if (flags & ~(uint32_t)(MKHOST_NO_TAR_DIGEST | MKHOST_FILE_DIGESTS))
             throw HostError("commit layers: only MKHOST_NO_TAR_DIGEST and MKHOST_FILE_DIGESTS are supported for a batch");
         m->fs.set_now(now_unix);
@@ -483,7 +496,7 @@ int mkhost_memfs_commit_layers_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_chu
         std::vector<BatchLayer> bl;
         for (size_t i = 0; i < n_layers; ++i)
             bl.push_back(BatchLayer{&maps[i], specs[i].tar_fd});
-        commit_layers_batch(eng, bl, n_threads, flags, outs, &m->fs, cache ? &cache->memo : nullptr, stats);
+        commit_layers_batch(engines, n_engines, bl, n_threads, flags, outs, &m->fs, cache ? &cache->memo : nullptr, stats);
         return 0;
     } catch (const std::exception &e) {
         set_err(err, errlen, std::string("failed to generate diff layers: ") + e.what());
@@ -861,8 +874,9 @@ struct CrcPacker {
     std::chrono::steady_clock::time_point t;
 
     // begins the session and leases its first arena
-    CrcPacker(mksnap_t *eng, int n_threads) : s(eng, n_threads, 1) // cap unrounded: CRC pieces end anywhere
+    CrcPacker(mksnap_t *eng, int n_threads, ReadPool &pool = ReadPool::get()) : s(eng, n_threads, 1) // cap unrounded: CRC pieces end anywhere
     {
+        s.pool = &pool;
         s.after_reads = [this]() {
             ms_reads += ms_since(t);
             t = std::chrono::steady_clock::now();
@@ -950,61 +964,120 @@ struct CrcPacker {
 
 extern "C" {
 
-static int context_crc32_impl(mksnap_t *eng, mkhost_crc_cache *cache, mkhost_crc_cache_stats *stats, const void *prefix,
-                              size_t prefix_len, const char *context_dir, const char *const *from_paths, size_t n_paths,
-                              int n_threads, uint32_t *crc_out, uint64_t *stream_len_out, char *err, size_t errlen)
+// The cacheID over n_engines engines (one engine: the whole stream in one session).  The context is walked once; every
+// segment's crc_suffix is its place in the whole stream, so each engine's crc_pure is its segments' share of the value
+// and the shares XOR.  Files that travel go to the engines by LPT over their bytes (largest first, each to the least
+// loaded engine); a path string or link target goes with the next file in walk order that travels, or to engine 0, as
+// do the prefix and every file the cache vouches for (mksnap_crc_add, no bytes).  Each engine packs on a thread of its
+// own with a reader pool of its own; the cache is read before they start and written after they have finished.
+static int context_crc32_impl(mksnap_t *const *engines, size_t n_engines, mkhost_crc_cache *cache, mkhost_crc_cache_stats *stats,
+                              const void *prefix, size_t prefix_len, const char *context_dir, const char *const *from_paths,
+                              size_t n_paths, int n_threads, uint32_t *crc_out, uint64_t *stream_len_out, char *err, size_t errlen)
 {
     try {
+        if (!engines || n_engines == 0 || !crc_out)
+            throw HostError("null argument");
+        for (size_t k = 0; k < n_engines; ++k)
+            if (!engines[k])
+                throw HostError("null argument");
         const auto t_start = std::chrono::steady_clock::now();
         std::vector<Seg> segs = context_segments(go_clean(context_dir), from_paths, n_paths, n_threads);
         const double ms_walk = ms_since(t_start);
         uint64_t total = prefix_len;
         for (const auto &g : segs)
             total += g.kind == 'F' ? g.size : g.bytes.size();
-        CrcPacker pk(eng, n_threads);
-        uint64_t after = total; // stream bytes not yet placed
-        auto put_text = [&](const void *p, size_t n) {
-            if (n) {
-                after -= n;
-                pk.text(p, n, after);
-            }
-        };
+        std::vector<uint64_t> after(segs.size()); // stream bytes behind each segment
+        std::vector<const mkhost_crc_cache::Entry *> hit(segs.size(), nullptr);
         mkhost_crc_cache_stats st{};
-        put_text(prefix, prefix_len);
-        for (const auto &g : segs) {
-            if (g.kind != 'F') {
-                put_text(g.bytes.data(), g.bytes.size());
+        std::vector<std::pair<uint64_t, size_t>> sent; // (bytes, segment) of every file that travels
+        uint64_t a = total - prefix_len;
+        for (size_t i = 0; i < segs.size(); ++i) {
+            const Seg &g = segs[i];
+            a -= g.kind == 'F' ? g.size : g.bytes.size();
+            after[i] = a;
+            if (g.kind != 'F')
                 continue;
-            }
             ++st.files_total;
             st.bytes_total += g.size;
-            after -= g.size;
             if (cache) { // unchanged since a build that remembered it: fold pure(content) in, send nothing
                 auto it = cache->files.find(g.path);
                 if (it != cache->files.end() && it->second.id == g.id) {
-                    ck(eng, mksnap_crc_add(eng, it->second.pure, g.size, after), "crc add");
+                    hit[i] = &it->second;
                     ++st.files_reused;
                     continue;
                 }
             }
             st.bytes_sent += g.size;
-            pk.file(g, after);
+            sent.emplace_back(g.size, i);
         }
-        pk.submit();
-        mksnap_result res;
-        const auto t_fin = std::chrono::steady_clock::now();
-        pk.finish(res);
-        if (getenv("MKHOST_TRACE")) // phase times on stderr
-            fprintf(stderr, "[mkhost] context crc32: %zu segments, %.1f MiB; walk %.2f ms, reads %.2f, acquire waits %.2f, submit %.2f, "
-                            "finish %.2f, total %.2f ms\n",
-                    segs.size(), (double)total / 1048576.0, ms_walk, pk.ms_reads, pk.ms_acquire, pk.ms_submit, ms_since(t_fin),
+        std::vector<size_t> owner(segs.size(), 0);
+        if (n_engines > 1) {
+            std::stable_sort(sent.begin(), sent.end(), [](const auto &x, const auto &y) { return x.first > y.first; });
+            std::vector<uint64_t> load(n_engines, 0);
+            for (const auto &f : sent) {
+                const size_t k = (size_t)(std::min_element(load.begin(), load.end()) - load.begin());
+                load[k] += f.first;
+                owner[f.second] = k;
+            }
+            size_t next = 0; // engine of the next file in walk order that travels
+            for (size_t i = segs.size(); i-- > 0;) {
+                if (segs[i].kind == 'F' && !hit[i])
+                    next = owner[i];
+                else
+                    owner[i] = segs[i].kind == 'F' ? 0 : next;
+            }
+        }
+        std::vector<std::vector<size_t>> mine(n_engines);
+        for (size_t i = 0; i < segs.size(); ++i)
+            mine[owner[i]].push_back(i);
+        std::vector<size_t> active{0}; // engine 0 and every engine with segments
+        for (size_t k = 1; k < n_engines; ++k)
+            if (!mine[k].empty())
+                active.push_back(k);
+        EngineThreads threads(active.size());
+        std::vector<std::unique_ptr<CrcPacker>> pks(active.size());
+        std::vector<mksnap_result> res(active.size());
+        threads.run([&](size_t j) {
+            mksnap_t *eng = engines[active[j]];
+            pks[j].reset(new CrcPacker(eng, n_threads, threads.pool(j)));
+            CrcPacker &pk = *pks[j];
+            if (j == 0 && prefix_len)
+                pk.text(prefix, prefix_len, total - prefix_len);
+            for (size_t i : mine[active[j]]) {
+                const Seg &g = segs[i];
+                if (g.kind != 'F') {
+                    if (!g.bytes.empty())
+                        pk.text(g.bytes.data(), g.bytes.size(), after[i]);
+                } else if (hit[i]) {
+                    ck(eng, mksnap_crc_add(eng, hit[i]->pure, g.size, after[i]), "crc add");
+                } else {
+                    pk.file(g, after[i]);
+                }
+            }
+            pk.submit();
+            pk.finish(res[j]);
+        });
+        mksnap_result all{};
+        for (const mksnap_result &r : res) {
+            all.crc_pure ^= r.crc_pure;
+            all.crc_bytes += r.crc_bytes;
+        }
+        if (getenv("MKHOST_TRACE")) { // phase times on stderr, summed over the engines
+            double ms_reads = 0, ms_acquire = 0, ms_submit = 0;
+            for (const auto &pk : pks)
+                ms_reads += pk->ms_reads, ms_acquire += pk->ms_acquire, ms_submit += pk->ms_submit;
+            fprintf(stderr, "[mkhost] context crc32: %zu segments, %.1f MiB, %zu engines; walk %.2f ms, reads %.2f, acquire waits %.2f, "
+                            "submit %.2f, total %.2f ms\n",
+                    segs.size(), (double)total / 1048576.0, active.size(), ms_walk, ms_reads, ms_acquire, ms_submit,
                     ms_since(t_start));
-        if (res.crc_bytes != total)
+        }
+        if (all.crc_bytes != total)
             throw HostError("internal: stream length mismatch");
-        *crc_out = mksnap_ctx_crc32(&res);
+        *crc_out = mksnap_ctx_crc32(&all);
         if (stream_len_out)
             *stream_len_out = total;
-        pk.remember(cache, nullptr);
+        for (const auto &pk : pks)
+            pk->remember(cache, nullptr);
         if (stats)
             *stats = st;
         return 0;
@@ -1018,7 +1091,7 @@ int mkhost_context_crc32(mksnap_t *eng, const void *prefix, size_t prefix_len, c
                          const char *const *from_paths, size_t n_paths, int n_threads, uint32_t *crc_out,
                          uint64_t *stream_len_out, char *err, size_t errlen)
 {
-    return context_crc32_impl(eng, nullptr, nullptr, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads, crc_out,
+    return context_crc32_impl(&eng, 1, nullptr, nullptr, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads, crc_out,
                               stream_len_out, err, errlen);
 }
 
@@ -1058,8 +1131,17 @@ int mkhost_context_crc32_cached(mksnap_t *eng, mkhost_crc_cache *cache, const vo
         set_err(err, errlen, "hash context sources: no cache object");
         return -1;
     }
-    return context_crc32_impl(eng, cache, stats, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads, crc_out,
+    return context_crc32_impl(&eng, 1, cache, stats, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads, crc_out,
                               stream_len_out, err, errlen);
+}
+
+int mkhost_context_crc32_multi(mksnap_t *const *engines, size_t n_engines, mkhost_crc_cache *cache, const void *prefix,
+                               size_t prefix_len, const char *context_dir, const char *const *from_paths, size_t n_paths,
+                               int n_threads, uint32_t *crc_out, uint64_t *stream_len_out, mkhost_crc_cache_stats *stats,
+                               char *err, size_t errlen)
+{
+    return context_crc32_impl(engines, n_engines, cache, stats, prefix, prefix_len, context_dir, from_paths, n_paths, n_threads,
+                              crc_out, stream_len_out, err, errlen);
 }
 
 // One engine session of mkhost_plan_cache_ids: the streams of the walked COPY/ADD steps `batch` (stream slot k = batch[k]).
