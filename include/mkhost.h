@@ -389,6 +389,32 @@ int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_
                                          size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
                                          mkhost_layer_cache_stats *stats, mkhost_gz_index_stats *gz_stats, char *err,
                                          size_t errlen);
+/* mkhost_memfs_update_from_tars_cached with the layers shared out over n_engines engines (see mkhost_context_crc32_multi
+ * for the threading).  On success the result equals that of mkhost_memfs_update_from_tars_cached(m, engines[0], lc, gz,
+ * keys, ...) with the same arguments: every outs[i] (DiffID, n_entries, tar_bytes, and the run's root / n_chunks /
+ * n_unique), the tree and its remembered file digests, stats, gz_stats, and the bytes mkhost_layer_cache_save and
+ * mkhost_gz_index_cache_save write afterwards; with n_engines == 1 it is that call, MKHOST_UNTAR included.
+ * Whole layers are assigned to the engines, by LPT over their blob lengths (fstat size; 0 for a pipe); the layers the
+ * layer cache replays are decided before any engine starts and need no engine, and ingested layers that share a key go to
+ * one engine.  Each engine ingests and finishes its share in a session of its own, on a thread of its own, with its
+ * DiffID streams in slots counted per engine (a share its engine cannot hold is refused before any engine reads or
+ * submits, and before the layer cache is touched).  The calling thread merges every layer into the tree in layer order
+ * once the engines are done.  Then one more session on engine 0 takes every engine's sorted-unique table and the
+ * replayed layers' chunk rows (mksnap_chunks_add) and its finish sorts, uniques and roots them: they must fit engine 0's
+ * max_chunks, else the call fails with that finish's MKSNAP_E_CAPACITY message (not a layer's) and the layer cache
+ * records nothing.  While the engines run, the caches are only read; an engine's gz lookups also
+ * see the entries its own earlier layers left in this call, and every entry is applied to gz in layer order afterwards.
+ * Every layer needs an fd of its own, since the layers are read at the same time.  If layer k is the lowest-indexed
+ * layer that fails (ingest or merge), the call returns -1 with the message the single call gives for it, layers before k
+ * stay merged, the layer cache records nothing and gz gets the entries of the layers up to k whose open succeeded; outs,
+ * the stats and the read positions of later layers' fds are unspecified.  Every engine stays usable.  Refused with more
+ * than one engine: MKHOST_UNTAR (the members are written to disk while they are read, so the layers cannot be read at the
+ * same time), and engines that cut under different CDC parameters. */
+int mkhost_memfs_update_from_tars_multi(mkhost_memfs *m, mksnap_t *const *engines, size_t n_engines, mkhost_layer_cache *lc,
+                                        mkhost_gz_index_cache *gz, const char *const *keys, int64_t now_unix,
+                                        const mkhost_tar_spec *layers, size_t n_layers, uint32_t flags,
+                                        mkhost_layer_result *outs, mkhost_layer_cache_stats *stats,
+                                        mkhost_gz_index_stats *gz_stats, char *err, size_t errlen);
 
 /* CopyOperation.Execute (lib/snapshot/copy_op.go:82-147) with fileio.Copier (lib/fileio/copy.go): what a COPY/ADD step
  * does to the file system when it runs with --modifyfs.  op->dst is used as the on-disk destination exactly like the

@@ -605,6 +605,14 @@ func (lc *LayerCache) Save(path string) error {
 // UpdateFromTarsCached is UpdateFromTarsIndexed that replays every layer lc remembers under its Key for an unchanged
 // store file and records the others; lc == nil is UpdateFromTarsIndexed.  Results are those of the uncached run.
 func (fs *MemFS) UpdateFromTarsCached(e *Engine, lc *LayerCache, gc *GzIndexCache, now int64, layers []TarLayer, untar bool, flags uint32) ([]LayerResult, error) {
+	return fs.UpdateFromTarsMulti([]*Engine{e}, lc, gc, now, layers, untar, flags)
+}
+
+// UpdateFromTarsMulti is UpdateFromTarsCached with the layers shared out over several engines -- one per GPU of the
+// build host, or several on one -- each driven by libmkhost from a thread of its own (mkhost_memfs_update_from_tars_multi).
+// The result is that of UpdateFromTarsCached on engines[0], bit for bit.  Every layer needs a File of its own, and untar
+// (--modifyfs) takes one engine.  The engines must not be used by anything else during the call.
+func (fs *MemFS) UpdateFromTarsMulti(engines []*Engine, lc *LayerCache, gc *GzIndexCache, now int64, layers []TarLayer, untar bool, flags uint32) ([]LayerResult, error) {
 	if untar {
 		flags |= 32 // MKHOST_UNTAR
 	}
@@ -641,8 +649,10 @@ func (fs *MemFS) UpdateFromTarsCached(e *Engine, lc *LayerCache, gc *GzIndexCach
 	var gst C.mkhost_gz_index_stats
 	errBuf := (*C.char)(C.malloc(errLen))
 	defer C.free(unsafe.Pointer(errBuf))
-	if rc := C.mkhost_memfs_update_from_tars_cached(fs.m, e.h, cache, gz, (**C.char)(unsafe.Pointer(ckeys)), C.int64_t(now),
-		&specs[0], C.size_t(n), C.uint32_t(flags), &outs[0], &st, &gst, errBuf, errLen); rc != 0 {
+	hs := engineArray(engines)
+	defer C.free(unsafe.Pointer(hs))
+	if rc := C.mkhost_memfs_update_from_tars_multi(fs.m, hs, C.size_t(len(engines)), cache, gz, (**C.char)(unsafe.Pointer(ckeys)),
+		C.int64_t(now), &specs[0], C.size_t(n), C.uint32_t(flags), &outs[0], &st, &gst, errBuf, errLen); rc != 0 {
 		return nil, fmt.Errorf("%s", C.GoString(errBuf))
 	}
 	res := make([]LayerResult, n)

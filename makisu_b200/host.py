@@ -142,6 +142,10 @@ SYMBOLS = [
                                                        C.POINTER(TarSpec), C.c_size_t, C.c_uint32, C.POINTER(LayerResult),
                                                        C.POINTER(LayerCacheStats), C.POINTER(GzIndexStats), C.c_char_p,
                                                        C.c_size_t]),
+    ("mkhost_memfs_update_from_tars_multi", C.c_int, [_P, C.POINTER(_P), C.c_size_t, _P, _P, C.POINTER(C.c_char_p),
+                                                      C.c_int64, C.POINTER(TarSpec), C.c_size_t, C.c_uint32,
+                                                      C.POINTER(LayerResult), C.POINTER(LayerCacheStats),
+                                                      C.POINTER(GzIndexStats), C.c_char_p, C.c_size_t]),
     ("mkhost_copy_op_execute", C.c_int, [C.POINTER(CopyOp), C.c_uint32, C.POINTER(C.c_char_p), C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_eval_symlinks", C.c_size_t, [C.c_char_p, C.c_char_p, C.c_char_p, C.c_size_t, C.c_char_p, C.c_size_t]),
     ("mkhost_cache_key", C.c_size_t, [C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]),
@@ -521,6 +525,18 @@ class MemFS:
         res = _run_layers(layers, keys, lambda specs, n, ks, outs, err: load().mkhost_memfs_update_from_tars_cached(
             self.h, eng.h, cache.h if cache is not None else None, gz.h if gz is not None else None, ks, now_unix, specs, n,
             flags, outs, C.byref(st), C.byref(gst), err, len(err)))
+        return (res, {k: getattr(st, k) for k, _ in LayerCacheStats._fields_},
+                {k: getattr(gst, k) for k, _ in GzIndexStats._fields_})
+
+    def update_from_tars_multi(self, engines: Sequence[abi.Engine], cache: Optional["LayerCache"],
+                               gz: Optional["GzIndexCache"], keys: Sequence, now_unix: int, layers: Sequence, flags: int = 0):
+        """update_from_tars_cached with whole layers sharded over several engines, each driven from a thread of its own
+        -> (dicts, layer-cache stats dict, gz-index stats dict).  The result is that of update_from_tars_cached on
+        engines[0]; every layer needs an fd of its own."""
+        st, gst, hs = LayerCacheStats(), GzIndexStats(), _engines(engines)
+        res = _run_layers(layers, keys, lambda specs, n, ks, outs, err: load().mkhost_memfs_update_from_tars_multi(
+            self.h, hs, len(engines), cache.h if cache is not None else None, gz.h if gz is not None else None, ks,
+            now_unix, specs, n, flags, outs, C.byref(st), C.byref(gst), err, len(err)))
         return (res, {k: getattr(st, k) for k, _ in LayerCacheStats._fields_},
                 {k: getattr(gst, k) for k, _ in GzIndexStats._fields_})
 

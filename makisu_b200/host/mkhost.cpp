@@ -707,6 +707,309 @@ int update_from_tars_impl(mkhost_memfs *m, mksnap_t *eng, int64_t now_unix, cons
     }
 }
 
+// mkhost_memfs_update_from_tars_multi (one engine: update_from_tars_impl).  Without MKHOST_UNTAR an ingest never touches the
+// tree, so whole layers go to the engines and only their merges keep the run's order:
+//  - On this thread, before any engine starts: the layer cache decides which layers are replayed (they need no engine
+//    until the end), and the ingested layers go to the engines by LPT over their blob lengths, the layers of one key
+//    together (a key's gz index entry is then read and written by one engine, in layer order).
+//  - Each engine ingests its share, ascending, in a session of its own on a thread of its own: DiffID streams in slots
+//    0..share-1 (MKSNAP_R_DEFER, with its own stream log), per-file streams behind them, their rows taken after each
+//    layer.  Its gz lookups see the entries its own earlier layers left, then the cache as the call found it.  An
+//    engine stops at its first failing layer.  Every engine finishes its own session on its own thread, so the
+//    engines' DiffID chains are hashed at the same time (each finish flushes its stream log), and hands over its
+//    DiffIDs, its computed chunk rows and its sorted-unique table.
+//  - Then this thread merges the layers in order up to the first that failed (ingest or merge), applies the gz entries
+//    of the layers up to that one in order, and reports that layer's failure, as the single call would have.
+//  - A last, short session on engine 0 takes every engine's unique table and the replayed layers' chunk rows
+//    (mksnap_chunks_add) and finishes: the run's root and n_unique.  Each engine's computed chunk rows go to its own
+//    layers through its own session coordinates, and the layer cache is written, as in the single call.
+int update_from_tars_sharded(mkhost_memfs *m, mksnap_t *const *engines, size_t n_engines, int64_t now_unix,
+                             const mkhost_tar_spec *layers, size_t n_layers, uint32_t flags, mkhost_layer_result *outs,
+                             GzIndexMap *cache, const char *const *keys, mkhost_gz_index_stats *stats, LayerMemo *lc,
+                             mkhost_layer_cache_stats *lstats, char *err, size_t errlen)
+{
+    try {
+        if (!m || !engines || n_engines == 0 || (!layers && n_layers) || (!outs && n_layers))
+            throw HostError("null argument");
+        for (size_t k = 0; k < n_engines; ++k)
+            if (!engines[k])
+                throw HostError("null argument");
+        if (flags & ~(uint32_t)(MKHOST_NO_TAR_DIGEST | MKHOST_FILE_DIGESTS | MKHOST_UNTAR))
+            throw HostError("update from tars: flags take MKHOST_NO_TAR_DIGEST, MKHOST_FILE_DIGESTS and MKHOST_UNTAR; "
+                            "MKHOST_GUNZIP goes per layer");
+        for (size_t i = 0; i < n_layers; ++i)
+            if (layers[i].flags & ~(uint32_t)MKHOST_GUNZIP)
+                throw HostError("update from tars: layer " + std::to_string(i) + ": only MKHOST_GUNZIP is a per-layer flag");
+        if (n_engines == 1)
+            return update_from_tars_impl(m, engines[0], now_unix, layers, n_layers, flags, MKSNAP_R_DEFER, outs, cache, keys,
+                                         stats, lc, lstats, "update memfs from tars: ", err, errlen);
+        if (flags & MKHOST_UNTAR)
+            throw HostError("update from tars: MKHOST_UNTAR writes the members while the layers are read, so it takes one engine");
+        check_same_cdc(engines, n_engines);
+        if (n_layers == 0)
+            return 0;
+        const bool want_digest = !(flags & MKHOST_NO_TAR_DIGEST);
+        const bool file_digests = (flags & MKHOST_FILE_DIGESTS) != 0;
+        // the layer cache is bound (and cleared when cut under other CDC parameters) only once nothing is refused; a
+        // cache that binding would clear replays nothing
+        mksnap_cdc_params cdc0;
+        ck(engines[0], mksnap_get_cdc(engines[0], &cdc0), "cdc parameters");
+        const bool lc_valid = lc && memcmp(&cdc0, &lc->cdc, sizeof cdc0) == 0;
+        mkhost_layer_cache_stats lst{};
+        lst.layers = n_layers;
+
+        // the plan: replayed layers, and the ingested ones shared out in units of one key
+        std::vector<const LayerMemo::Entry *> hit(n_layers, nullptr);
+        std::vector<FileId> id(n_layers);
+        std::vector<bool> cacheable(n_layers, false);
+        std::vector<uint64_t> unit_weight;
+        std::vector<std::vector<size_t>> unit_layers;
+        std::map<std::string, size_t> unit_of_key;
+        for (size_t i = 0; i < n_layers; ++i) {
+            const char *key = keys ? keys[i] : nullptr;
+            cacheable[i] = lc && key && layer_file_id(layers[i].tar_fd, &id[i]);
+            hit[i] = cacheable[i] && lc_valid ? lc->find(key, id[i], flags | layers[i].flags) : nullptr;
+            if (hit[i])
+                continue;
+            struct stat st;
+            const uint64_t w = fstat(layers[i].tar_fd, &st) == 0 && S_ISREG(st.st_mode) ? (uint64_t)st.st_size : 0;
+            size_t u = unit_weight.size();
+            if (key) {
+                auto ins = unit_of_key.emplace(key, u);
+                u = ins.first->second;
+            }
+            if (u == unit_weight.size()) {
+                unit_weight.push_back(0);
+                unit_layers.emplace_back();
+            }
+            unit_weight[u] += w;
+            unit_layers[u].push_back(i);
+        }
+        const std::vector<std::vector<size_t>> unit_share = lpt_shares(unit_weight, n_engines);
+
+        struct Shard {
+            std::vector<size_t> ingests; // its layers, ascending: local stream slot j <-> ingests[j]
+            std::vector<uint64_t> at{0}; // where ingests[j]'s submitted bytes start in the session's chunk-end coordinates
+            uint32_t max_files = 0;      // most per-file streams of one of its layers so far
+            GzIndexMap own;              // gz entries its layers left in this call
+            mkhost_gz_index_stats gst{};
+            mksnap_result res{};
+            std::vector<uint8_t> rows, dig, table; // DiffID rows; computed chunk digests (with ends) and unique table
+            std::vector<uint64_t> ends;
+            std::exception_ptr failed;             // a failure that belongs to no layer (finish, chunk table)
+        };
+        std::vector<Shard> sh(n_engines);
+        for (size_t k = 0; k < n_engines; ++k) {
+            for (size_t u : unit_share[k])
+                sh[k].ingests.insert(sh[k].ingests.end(), unit_layers[u].begin(), unit_layers[u].end());
+            std::sort(sh[k].ingests.begin(), sh[k].ingests.end());
+        }
+        size_t n_used = 1; // engines given nothing stay untouched; engine 0 always finishes the run
+        for (size_t k = 1; k < n_engines; ++k)
+            if (!sh[k].ingests.empty())
+                n_used = k + 1;
+        for (size_t k = 0; k < n_used; ++k) {
+            if (sh[k].ingests.empty())
+                continue;
+            const mksnap_limits lim = engine_limits(engines[k]);
+            const size_t L = sh[k].ingests.size();
+            if (L + (file_digests ? 1 : 0) > lim.max_streams)
+                throw HostError("engine " + std::to_string(k) + "'s share of " + std::to_string(L) +
+                                " layers needs a stream slot per layer" + (file_digests ? " and more for the per-file digests" : "") +
+                                ": engine max_extents (" + std::to_string(lim.max_streams) + ") is too small");
+        }
+        m->fs.set_now(now_unix);
+        if (lc)
+            lc->bind(engines[0]);
+
+        struct Layer {
+            IngestedLayer in;
+            std::vector<uint8_t> file_rows; // its per-file digests, member order
+            std::unique_ptr<GzIndexMap::Entry> gz;
+            bool ran = false;
+            std::string failed;
+        };
+        std::vector<Layer> lay(n_layers);
+        for (size_t i = 0; i < n_layers; ++i)
+            lay[i].ran = hit[i] != nullptr; // a replayed layer has nothing to run before its merge
+        EngineThreads threads(n_used);
+        threads.run([&](size_t k) {
+            Shard &s = sh[k];
+            if (s.ingests.empty())
+                return;
+            mksnap_t *eng = engines[k];
+            const uint32_t file_base = (uint32_t)s.ingests.size();
+            try {
+                ck(eng, mksnap_begin(eng), "begin");
+                if (want_digest)
+                    ck(eng, mksnap_reserve_stream_log(eng, RUN_STREAM_LOG_BYTES), "reserve stream log");
+            } catch (const std::exception &e) { // the first layer's failure, as in the single call
+                lay[s.ingests[0]].failed = e.what();
+                return;
+            }
+            for (size_t j = 0; j < s.ingests.size(); ++j) {
+                const size_t i = s.ingests[j];
+                Layer &l = lay[i];
+                try {
+                    const char *key = keys ? keys[i] : nullptr;
+                    const GzIndexUse ix{&s.own, key, &s.gst, cache};
+                    ingest_layer(m->fs, eng, layers[i].tar_fd, flags | layers[i].flags, (uint32_t)j, MKSNAP_R_DEFER, file_base, l.in,
+                                 cache && key ? &ix : nullptr);
+                    if (l.in.gz_indexed)
+                        l.gz.reset(new GzIndexMap::Entry(s.own.e[key]));
+                    if (l.in.n_file_streams) { // inline streams: their rows are final once the submits so far have run
+                        s.max_files = std::max(s.max_files, l.in.n_file_streams);
+                        std::vector<uint8_t> d(32 * ((uint64_t)file_base + s.max_files));
+                        ck(eng, mksnap_get_stream_digests(eng, d.data(), d.size() / 32), "stream digests");
+                        l.file_rows.assign(d.begin() + 32 * file_base, d.begin() + 32 * ((uint64_t)file_base + l.in.n_file_streams));
+                    }
+                    s.at.push_back(s.at.back() + l.in.submitted);
+                    l.ran = true;
+                } catch (const std::exception &e) {
+                    if (l.in.gz_indexed && !l.gz)
+                        l.gz.reset(new GzIndexMap::Entry(s.own.e[keys[i]]));
+                    l.failed = e.what();
+                    return;
+                }
+            }
+            try {
+                ck(eng, mksnap_finish(eng, &s.res), "finish");
+                s.rows.assign(32 * std::max<uint64_t>(s.res.n_streams, file_base), 0);
+                if (want_digest && !s.rows.empty())
+                    ck(eng, mksnap_get_stream_digests(eng, s.rows.data(), s.rows.size() / 32), "stream digests");
+                s.ends.resize(std::max<uint64_t>(1, s.res.n_chunks));
+                s.dig.resize(32 * s.ends.size());
+                if (lc && s.res.n_chunks)
+                    ck(eng, mksnap_get_chunks(eng, s.ends.data(), s.dig.data(), s.res.n_chunks), "chunk table");
+                s.table.resize(32 * s.res.n_unique);
+                if (s.res.n_unique)
+                    ck(eng, mksnap_get_table(eng, s.table.data(), s.res.n_unique), "chunk table");
+            } catch (...) {
+                s.failed = std::current_exception();
+            }
+        });
+
+        // merge in layer order, up to the first layer that failed
+        std::vector<uint64_t> entries(n_layers, 0);
+        size_t first_bad = n_layers;
+        std::string why;
+        for (size_t i = 0; i < n_layers && first_bad == n_layers; ++i) {
+            Layer &l = lay[i];
+            if (!l.ran) {
+                first_bad = i;
+                why = l.failed;
+                break;
+            }
+            try {
+                IngestedLayer replay;
+                if (hit[i])
+                    replay.members = hit[i]->members;
+                const std::map<std::string, MemFile> merged =
+                    hit[i] ? merge_layer(m->fs, flags, replay, hit[i]->file_digests.data(), 0) : merge_layer(m->fs, flags, l.in, l.file_rows.data(), 0);
+                entries[i] = merged.size();
+            } catch (const std::exception &e) {
+                first_bad = i;
+                why = e.what();
+            }
+        }
+        if (cache)
+            for (size_t i = 0; i < n_layers && i <= first_bad; ++i)
+                if (lay[i].gz)
+                    cache->e[keys[i]] = std::move(*lay[i].gz);
+        if (first_bad < n_layers)
+            throw HostError(why);
+        for (size_t k = 0; k < n_used; ++k)
+            if (sh[k].failed)
+                std::rethrow_exception(sh[k].failed);
+        if (stats)
+            for (const Shard &s : sh) {
+                stats->blobs += s.gst.blobs;
+                stats->blobs_with_index += s.gst.blobs_with_index;
+                stats->points_given += s.gst.points_given;
+                stats->points_linked += s.gst.points_linked;
+                stats->points_recorded += s.gst.points_recorded;
+            }
+
+        // One more session on engine 0 holds the run's table: every engine's unique rows and the replayed layers' rows.
+        // Its finish sorts, uniques and roots them, so root and n_unique are those of one table over the run; n_chunks
+        // counts every engine's computed chunks and every replayed row, as the single call's table does.
+        mksnap_t *eng0 = engines[0];
+        std::vector<const std::vector<uint8_t> *> tables;
+        for (size_t k = 0; k < n_used; ++k)
+            tables.push_back(&sh[k].table);
+        for (size_t i = 0; i < n_layers; ++i)
+            if (hit[i])
+                tables.push_back(&hit[i]->chunks);
+        ck(eng0, mksnap_begin(eng0), "begin");
+        for (const std::vector<uint8_t> *rows : tables) {
+            const uint64_t n = rows->size() / 32;
+            for (uint64_t r0 = 0; r0 < n; r0 += MKSNAP_CHUNKS_ADD_MAX)
+                ck(eng0, mksnap_chunks_add(eng0, rows->data() + 32 * r0, std::min<uint64_t>(MKSNAP_CHUNKS_ADD_MAX, n - r0)),
+                   "chunks add");
+        }
+        mksnap_result res;
+        ck(eng0, mksnap_finish(eng0, &res), "finish");
+        res.n_chunks = 0;
+        for (size_t k = 0; k < n_used; ++k)
+            res.n_chunks += sh[k].res.n_chunks;
+        for (size_t i = 0; i < n_layers; ++i)
+            if (hit[i])
+                res.n_chunks += hit[i]->chunks.size() / 32;
+
+        std::vector<std::unique_ptr<LayerMemo::Entry>> recording(n_layers);
+        for (size_t k = 0; k < n_used; ++k) {
+            const Shard &s = sh[k];
+            for (size_t j = 0; j < s.ingests.size(); ++j) {
+                const size_t i = s.ingests[j];
+                const IngestedLayer &in = lay[i].in;
+                set_layer_result(&outs[i], res, want_digest ? s.rows.data() + 32 * j : nullptr, entries[i], in.tar_bytes);
+                lst.blob_bytes_read += in.blob_bytes;
+                if (!cacheable[i])
+                    continue;
+                recording[i].reset(new LayerMemo::Entry);
+                LayerMemo::Entry &r = *recording[i];
+                r.id = id[i];
+                r.gunzip = (layers[i].flags & MKHOST_GUNZIP) != 0;
+                r.has_diffid = want_digest;
+                r.has_file_digests = file_digests;
+                r.tar_bytes = in.tar_bytes;
+                r.members = std::move(lay[i].in.members);
+                r.file_digests = std::move(lay[i].file_rows);
+                if (want_digest)
+                    memcpy(r.diffid.data(), s.rows.data() + 32 * j, 32);
+            }
+            if (!lc)
+                continue;
+            // Every ingested layer submitted arenas of its own, so the chunks it computed end inside its share of this
+            // engine's session bytes, (at[j], at[j + 1]].
+            for (uint64_t c = 0; c < s.res.n_chunks; ++c) {
+                if (s.ends[c] == 0 || s.ends[c] > s.at.back())
+                    throw HostError("internal: the chunk table does not match the layers submitted");
+                const size_t j = std::upper_bound(s.at.begin(), s.at.end(), s.ends[c] - 1) - s.at.begin() - 1;
+                if (recording[s.ingests[j]])
+                    recording[s.ingests[j]]->chunks.insert(recording[s.ingests[j]]->chunks.end(), s.dig.begin() + 32 * c,
+                                                           s.dig.begin() + 32 * (c + 1));
+            }
+        }
+        for (size_t i = 0; i < n_layers; ++i) {
+            if (hit[i]) {
+                set_layer_result(&outs[i], res, want_digest ? hit[i]->diffid.data() : nullptr, entries[i], hit[i]->tar_bytes);
+                lst.layers_replayed++;
+                lst.chunks_appended += hit[i]->chunks.size() / 32;
+            } else if (recording[i]) {
+                lc->e[keys[i]] = std::move(*recording[i]);
+                lst.layers_recorded++;
+            }
+        }
+        if (lstats)
+            *lstats = lst;
+        return 0;
+    } catch (const std::exception &e) {
+        set_err(err, errlen, std::string("update memfs from tars: ") + e.what());
+        return -1;
+    }
+}
+
 } // namespace
 
 extern "C" {
@@ -752,6 +1055,16 @@ int mkhost_memfs_update_from_tars_cached(mkhost_memfs *m, mksnap_t *eng, mkhost_
 {
     return update_from_tars_impl(m, eng, now_unix, layers, n_layers, flags, MKSNAP_R_DEFER, outs, gz ? &gz->map : nullptr,
                                  keys, gz_stats, lc ? &lc->memo : nullptr, stats, "update memfs from tars: ", err, errlen);
+}
+
+int mkhost_memfs_update_from_tars_multi(mkhost_memfs *m, mksnap_t *const *engines, size_t n_engines, mkhost_layer_cache *lc,
+                                        mkhost_gz_index_cache *gz, const char *const *keys, int64_t now_unix,
+                                        const mkhost_tar_spec *layers, size_t n_layers, uint32_t flags,
+                                        mkhost_layer_result *outs, mkhost_layer_cache_stats *stats,
+                                        mkhost_gz_index_stats *gz_stats, char *err, size_t errlen)
+{
+    return update_from_tars_sharded(m, engines, n_engines, now_unix, layers, n_layers, flags, outs, gz ? &gz->map : nullptr,
+                                    keys, gz_stats, lc ? &lc->memo : nullptr, stats, err, errlen);
 }
 
 mkhost_layer_cache *mkhost_layer_cache_new(void) { return new mkhost_layer_cache; }
